@@ -339,11 +339,17 @@ LADI_API int ladi_vae_encode(ladi_engine* engine, const void* x_nhwc8, int batch
  * order with their encoder layer indices int_layers[] (vae.py:183-212; n_feats = 0: plain decode) -> image NHWC fp32 [batch, 8h, 8w, 4]. */
 LADI_API int ladi_vae_decode_emasc(ladi_engine* engine, const void* z_nhwc8, int batch, int lat_h, int lat_w, const void* const* feats, int n_feats,
                                    const int* int_layers, float* image_out, void* workspace, int64_t workspace_bytes, void* stream);
-/* per scale i: outs[i] = conv3x3(silu(conv3x3(feats[i]))) * inv_masks[i] (fp32 per output pixel = 1 - nearest-resized mask; NULL: no
- * masking); feats / outs NHWC bf16 at resolution (height, width) / emasc_stride[i]. */
+/* per scale i: outs[i] = conv(silu(conv(feats[i]))) * inv_masks[i] (fp32 per output pixel = 1 - nearest-resized mask; NULL: no
+ * masking); feats / outs NHWC bf16 at resolution (height, width) / emasc_stride[i].  The form of each scale is read from the weight table
+ * (emasc.py:20-33): with `emasc.<i>.w1/b1` and `emasc.<i>.w2/b2` it is the nonlinear form above; without `emasc.<i>.w2` it is the linear
+ * form, outs[i] = conv(feats[i]) * inv_masks[i] with `emasc.<i>.w1/b1`.  The kernel size comes from the packed width of `emasc.<i>.w1`:
+ * cols / (64 * ceil(emasc_in[i] / 64)) taps, 9 -> 3x3 with padding 1, 1 -> 1x1 with padding 0; any other width is rejected. */
 LADI_API int ladi_emasc_forward(ladi_engine* engine, const void* const* feats, const float* const* inv_masks, int batch, int height, int width,
                                 void* const* outs, void* workspace, int64_t workspace_bytes, void* stream);
-/* feats bf16 [batch, tokens, adapter_dim] (CLIP ViT-H last_hidden_state) -> out bf16 [batch, adapter_out] */
+/* feats bf16 [batch, tokens, adapter_dim] (CLIP ViT-H last_hidden_state) -> out bf16 [batch, adapter_out].  The number of encoder layers
+ * L is read from the weight table (inversion_adapter.py:9): layers 0..L-2 are `adapter.enc<l>.{ln1,qkv,o,ln2,fc1,fc2}` (full pre-LN
+ * CLIP layers over all tokens, attention on ladi_attention_small, tokens <= 1024), counted from l = 0 while `adapter.enc<l>.ln1.0`
+ * exists; the last layer keeps the names `adapter.{ln1,kv,q,o,ln2,fc1,fc2}` and runs on the CLS row only. */
 LADI_API int ladi_inversion_adapter_forward(ladi_engine* engine, const void* feats, int batch, int tokens, void* out, void* workspace,
                                             int64_t workspace_bytes, void* stream);
 /* n_steps x (ladi_unet_forward + ladi_ddim_cfg_step) enqueued on `stream`: unet_in NHWC bf16 [cfg ? 2*batch : batch, h, w, in_pitch] with

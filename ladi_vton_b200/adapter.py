@@ -1,15 +1,18 @@
 """H100-native InversionAdapter -- drop-in for the reference's src/models/inversion_adapter.py:5-28 built with the dims of
 hubconf.py:16-27 (CLIP ViT-H vision hidden 1280, 16 heads of 80, MLP 5120; projection 1280 -> 5120 -> 5120 -> 16384) and called at
-src/inference.py:276-277.  State-dict keys: encoder_layers.0.{self_attn.{q,k,v,out}_proj, layer_norm1, mlp.fc1, mlp.fc2, layer_norm2},
-post_layernorm, layers.{0,3,6}.
+src/inference.py:276-277.  State-dict keys: encoder_layers.{l}.{self_attn.{q,k,v,out}_proj, layer_norm1, mlp.fc1, mlp.fc2, layer_norm2}
+for l < num_encoder_layers, post_layernorm, layers.{0,3,6}.
 
-Only the CLS row of the encoder layer's output is consumed (inversion_adapter.py:26), so after LayerNorm-1 and the K/V projection of
-all 257 tokens, everything (query, attention, out-proj, MLP, projection head) runs on one row per image: 136 M weights are read once
-per call -- an HBM-bound chain of GEMMs on the wgmma kernel with GELU(erf) / residual epilogues.
+The release checkpoints have one encoder layer; the training scripts (train_inversion_adapter.py, train_vto.py `--num_encoder_layers`)
+can make more.  Layers 0..L-2 are full CLIP encoder layers over all 257 tokens (the arithmetic of clip.encoder_layer).  Only the CLS
+row of the last layer's output is consumed (inversion_adapter.py:26), so after its LayerNorm-1 and the K/V projection of all tokens,
+everything (query, attention, out-proj, MLP, projection head) runs on one row per image: 136 M weights are read once per call -- an
+HBM-bound chain of GEMMs on the wgmma kernel with GELU(erf) / residual epilogues.
 """
 import torch
 
 from . import engine as eng, lib, ops
+from .clip import encoder_layer, encoder_layer_shapes, pack_encoder_layer
 from .weights import f32, pack_linear
 
 
@@ -18,8 +21,9 @@ class InversionAdapter:
         if config is not None:  # accept the reference's `config=config.vision_config`
             heads = getattr(config, "num_attention_heads", heads)
             mlp_dim = getattr(config, "intermediate_size", mlp_dim)
-        if num_encoder_layers != 1:
-            raise NotImplementedError("the reference hub constructor uses exactly one encoder layer (hubconf.py:22)")
+        if int(num_encoder_layers) < 1:
+            raise ValueError(f"num_encoder_layers must be >= 1, got {num_encoder_layers}")
+        self.num_encoder_layers = int(num_encoder_layers)
         self.dim, self.hidden, self.out_dim, self.heads, self.mlp_dim = input_dim, hidden_dim, output_dim, heads, mlp_dim
         self.device = torch.device("cpu")
         self._sd, self.P = None, None
@@ -32,13 +36,8 @@ class InversionAdapter:
 
     def param_shapes(self):
         d, S = self.dim, {}
-        e = "encoder_layers.0."
-        for n in ("q_proj", "k_proj", "v_proj", "out_proj"):
-            S[e + f"self_attn.{n}.weight"], S[e + f"self_attn.{n}.bias"] = (d, d), (d,)
-        for n in ("layer_norm1", "layer_norm2"):
-            S[e + n + ".weight"], S[e + n + ".bias"] = (d,), (d,)
-        S[e + "mlp.fc1.weight"], S[e + "mlp.fc1.bias"] = (self.mlp_dim, d), (self.mlp_dim,)
-        S[e + "mlp.fc2.weight"], S[e + "mlp.fc2.bias"] = (d, self.mlp_dim), (d,)
+        for l in range(self.num_encoder_layers):
+            encoder_layer_shapes(S, f"encoder_layers.{l}.", d, self.mlp_dim)
         S["post_layernorm.weight"], S["post_layernorm.bias"] = (d,), (d,)
         S["layers.0.weight"], S["layers.0.bias"] = (self.hidden, d), (self.hidden,)
         S["layers.3.weight"], S["layers.3.bias"] = (self.hidden, self.hidden), (self.hidden,)
@@ -69,8 +68,11 @@ class InversionAdapter:
 
     def _pack(self):
         g = lambda k: self._sd[k].to(self.device, torch.float32)
-        e = "encoder_layers.0."
+        L = self.num_encoder_layers
+        e = f"encoder_layers.{L - 1}."
         P = {}
+        for l in range(L - 1):  # full-sequence layers; the last one is packed below for its CLS-row form
+            pack_encoder_layer(P, f"enc{l}.", g, f"encoder_layers.{l}.")
         P["ln1"] = (f32(g(e + "layer_norm1.weight")), f32(g(e + "layer_norm1.bias")))
         P["ln2"] = (f32(g(e + "layer_norm2.weight")), f32(g(e + "layer_norm2.bias")))
         P["lnp"] = (f32(g("post_layernorm.weight")), f32(g("post_layernorm.bias")))
@@ -96,6 +98,11 @@ class InversionAdapter:
             ws = self.engine.workspace(eng.MODULE_ADAPTER, B, T, 0)
             lib.call("ladi_inversion_adapter_forward", self.engine.h, ops._ptr(xb), B, T, ops._ptr(out), ops._ptr(ws), ws.numel(), ops._stream())
             return out
+        if self.num_encoder_layers > 1:
+            xt = xb.view(B * T, d)
+            for l in range(self.num_encoder_layers - 1):
+                xt = encoder_layer(P, f"enc{l}.", xt, B, T, self.heads, self.mlp_dim, 1e-5)
+            xb = xt.view(B, T, d)
         y = ops.layernorm(xb.view(B * T, d), *P["ln1"])                                  # pre-LN over all tokens
         kv = ops.gemm(y, P["kv.w"], 2 * d, bias=P["kv.b"]).view(B, T, 2 * d)
         y0 = y.view(B, T, d)[:, 0]                                                      # CLS rows, pitch T*d

@@ -84,38 +84,50 @@ class _Tower:
                 self._pack()
         return self
 
-    def _layer_shapes(self, S, p, d, mlp):
-        for n in ("q_proj", "k_proj", "v_proj", "out_proj"):
-            S[p + f"self_attn.{n}.weight"], S[p + f"self_attn.{n}.bias"] = (d, d), (d,)
-        for n in ("layer_norm1", "layer_norm2"):
-            S[p + n + ".weight"], S[p + n + ".bias"] = (d,), (d,)
-        S[p + "mlp.fc1.weight"], S[p + "mlp.fc1.bias"] = (mlp, d), (mlp,)
-        S[p + "mlp.fc2.weight"], S[p + "mlp.fc2.bias"] = (d, mlp), (d,)
-
     def _pack_layers(self, P):
         g = lambda k: self._sd[k].to(self.device, torch.float32)
         for i in range(self.config.num_hidden_layers):
             p = f"{self.prefix}.encoder.layers.{i}."
-            P[p + "ln1"] = (f32(g(p + "layer_norm1.weight")), f32(g(p + "layer_norm1.bias")))
-            P[p + "ln2"] = (f32(g(p + "layer_norm2.weight")), f32(g(p + "layer_norm2.bias")))
-            P[p + "qkv.w"] = pack_linear(torch.cat([g(p + f"self_attn.{n}_proj.weight") for n in "qkv"]))
-            P[p + "qkv.b"] = f32(torch.cat([g(p + f"self_attn.{n}_proj.bias") for n in "qkv"]))
-            for n, k in (("o", "self_attn.out_proj"), ("fc1", "mlp.fc1"), ("fc2", "mlp.fc2")):
-                P[p + n + ".w"], P[p + n + ".b"] = pack_linear(g(p + k + ".weight")), f32(g(p + k + ".bias"))
+            pack_encoder_layer(P, p, g, p)
 
     def _stack(self, x, B, T, causal):
         """x [B*T, C] bf16 -> [B*T, C] bf16 through all encoder layers (transformers CLIPEncoderLayer: pre-LN, residual adds)."""
-        P, cfg = self.P, self.config
-        C, heads, mlp = cfg.hidden_size, cfg.num_attention_heads, cfg.intermediate_size
-        scale = (C // heads) ** -0.5
+        cfg = self.config
         for i in range(cfg.num_hidden_layers):
-            p = f"{self.prefix}.encoder.layers.{i}."
-            qkv = ops.gemm(ops.layernorm(x, *P[p + "ln1"], eps=cfg.layer_norm_eps), P[p + "qkv.w"], 3 * C, bias=P[p + "qkv.b"]).view(B, T, 3 * C)
-            a = ops.attention_small(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], heads, scale, causal=causal)
-            x = ops.gemm(a.view(B * T, C), P[p + "o.w"], C, bias=P[p + "o.b"], residual=x)
-            h = ops.gemm(ops.layernorm(x, *P[p + "ln2"], eps=cfg.layer_norm_eps), P[p + "fc1.w"], mlp, bias=P[p + "fc1.b"], act=ops.ACT_GELU)
-            x = ops.gemm(h, P[p + "fc2.w"], C, bias=P[p + "fc2.b"], residual=x)
+            x = encoder_layer(self.P, f"{self.prefix}.encoder.layers.{i}.", x, B, T, cfg.num_attention_heads, cfg.intermediate_size,
+                              cfg.layer_norm_eps, causal)
         return x
+
+
+# ---- one CLIP encoder layer: shared by both towers and by the inversion adapter's full-sequence layers -----------------------------
+def encoder_layer_shapes(S, p, d, mlp):
+    """transformers CLIPEncoderLayer state-dict entries under prefix `p`."""
+    for n in ("q_proj", "k_proj", "v_proj", "out_proj"):
+        S[p + f"self_attn.{n}.weight"], S[p + f"self_attn.{n}.bias"] = (d, d), (d,)
+    for n in ("layer_norm1", "layer_norm2"):
+        S[p + n + ".weight"], S[p + n + ".bias"] = (d,), (d,)
+    S[p + "mlp.fc1.weight"], S[p + "mlp.fc1.bias"] = (mlp, d), (mlp,)
+    S[p + "mlp.fc2.weight"], S[p + "mlp.fc2.bias"] = (d, mlp), (d,)
+
+
+def pack_encoder_layer(P, dst, g, src):
+    """State-dict entries under `src` (read through g(key) -> fp32 device tensor) -> packed entries P[dst + {ln1, ln2, qkv.*, o.*, fc1.*, fc2.*}]."""
+    P[dst + "ln1"] = (f32(g(src + "layer_norm1.weight")), f32(g(src + "layer_norm1.bias")))
+    P[dst + "ln2"] = (f32(g(src + "layer_norm2.weight")), f32(g(src + "layer_norm2.bias")))
+    P[dst + "qkv.w"] = pack_linear(torch.cat([g(src + f"self_attn.{n}_proj.weight") for n in "qkv"]))
+    P[dst + "qkv.b"] = f32(torch.cat([g(src + f"self_attn.{n}_proj.bias") for n in "qkv"]))
+    for n, k in (("o", "self_attn.out_proj"), ("fc1", "mlp.fc1"), ("fc2", "mlp.fc2")):
+        P[dst + n + ".w"], P[dst + n + ".b"] = pack_linear(g(src + k + ".weight")), f32(g(src + k + ".bias"))
+
+
+def encoder_layer(P, p, x, B, T, heads, mlp, eps, causal=False):
+    """x [B*T, C] bf16 -> [B*T, C] bf16 through the packed layer P[p + ...] (transformers CLIPEncoderLayer: pre-LN, residual adds)."""
+    C = x.shape[1]
+    qkv = ops.gemm(ops.layernorm(x, *P[p + "ln1"], eps=eps), P[p + "qkv.w"], 3 * C, bias=P[p + "qkv.b"]).view(B, T, 3 * C)
+    a = ops.attention_small(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], heads, (C // heads) ** -0.5, causal=causal)
+    x = ops.gemm(a.view(B * T, C), P[p + "o.w"], C, bias=P[p + "o.b"], residual=x)
+    h = ops.gemm(ops.layernorm(x, *P[p + "ln2"], eps=eps), P[p + "fc1.w"], mlp, bias=P[p + "fc1.b"], act=ops.ACT_GELU)
+    return ops.gemm(h, P[p + "fc2.w"], C, bias=P[p + "fc2.b"], residual=x)
 
 
 SD2_TEXT_ENCODER = dict(vocab_size=49408, hidden_size=1024, intermediate_size=4096, num_hidden_layers=23, num_attention_heads=16,
@@ -140,7 +152,7 @@ class CLIPTextModel(_Tower):
         S["text_model.embeddings.token_embedding.weight"] = (c.vocab_size, d)
         S["text_model.embeddings.position_embedding.weight"] = (c.max_position_embeddings, d)
         for i in range(c.num_hidden_layers):
-            self._layer_shapes(S, f"text_model.encoder.layers.{i}.", d, c.intermediate_size)
+            encoder_layer_shapes(S, f"text_model.encoder.layers.{i}.", d, c.intermediate_size)
         S["text_model.final_layer_norm.weight"], S["text_model.final_layer_norm.bias"] = (d,), (d,)
         return S
 
@@ -220,7 +232,7 @@ class CLIPVisionModelWithProjection(_Tower):
         for n in ("pre_layrnorm", "post_layernorm"):
             S[f"vision_model.{n}.weight"], S[f"vision_model.{n}.bias"] = (d,), (d,)
         for i in range(c.num_hidden_layers):
-            self._layer_shapes(S, f"vision_model.encoder.layers.{i}.", d, c.intermediate_size)
+            encoder_layer_shapes(S, f"vision_model.encoder.layers.{i}.", d, c.intermediate_size)
         return S
 
     def _pack(self):

@@ -654,24 +654,90 @@ void vae_decode(Ctx& c, const T& zin, const T* feats, int n_feats, const int* in
   c.drop(hn);
 }
 
-// EMASC (emasc.py:25-40): per scale conv3x3 -> SiLU -> conv3x3, mask_features' (1 - mask) as the second conv's row scale
+// EMASC (emasc.py:20-33,37-40): per scale either the nonlinear form conv -> SiLU -> conv, or (no `emasc.%d.w2` in the weight table) the
+// linear form, one conv.  mask_features' (1 - mask) is the row scale of the last conv.  The kernel size is read from the packed width of
+// `emasc.%d.w1` (taps x 64-padded input channels): 9 taps -> 3x3 with padding 1, 1 tap -> 1x1 with padding 0.
 void emasc_forward(Ctx& c, const T* feats, const float* const* inv_masks, int n, const T* outs) {
   for (int i = 0; i < n && c.ok(); ++i) {
+    const Weight& w1 = c.W(fmt("emasc.%d.w1", i));
+    if (!c.ok()) return;
+    const int cin = c.e->cfg.emasc_in[i], kpad = (cin + 63) / 64 * 64;
+    const int taps = w1.cols % kpad == 0 ? w1.cols / kpad : 0;
+    if (taps != 9 && taps != 1) { c.fail("engine: emasc.%d.w1 is %d wide: not a 3x3 or 1x1 kernel over %d channels", i, w1.cols, cin); return; }
+    const int k = taps == 9 ? 3 : 1;
+    const bool linear = c.e->w.find(fmt("emasc.%d.w2", i)) == c.e->w.end();
+    const float* rs = inv_masks != nullptr ? inv_masks[i] : nullptr;
     ConvOpt o1;
-    o1.bias = c.F(fmt("emasc.%d.b1", i)); o1.act = LADI_ACT_SILU;
-    T t = c.conv(&feats[i], nullptr, c.W(fmt("emasc.%d.w1", i)), c.e->cfg.emasc_in[i], o1);
+    o1.ksize = k; o1.pad_lo = k / 2; o1.bias = c.F(fmt("emasc.%d.b1", i));
+    if (linear) {
+      o1.row_scale = rs; o1.out = &outs[i];
+      c.conv(&feats[i], nullptr, w1, c.e->cfg.emasc_out[i], o1);
+      continue;
+    }
+    o1.act = LADI_ACT_SILU;
+    T t = c.conv(&feats[i], nullptr, w1, cin, o1);
     ConvOpt o2;
-    o2.bias = c.F(fmt("emasc.%d.b2", i)); o2.row_scale = inv_masks != nullptr ? inv_masks[i] : nullptr; o2.out = &outs[i];
-    const T ts = t.slice(0, c.e->cfg.emasc_in[i]);
+    o2.ksize = k; o2.pad_lo = k / 2; o2.bias = c.F(fmt("emasc.%d.b2", i)); o2.row_scale = rs; o2.out = &outs[i];
+    const T ts = t.slice(0, cin);
     c.conv(&ts, nullptr, c.W(fmt("emasc.%d.w2", i)), c.e->cfg.emasc_out[i], o2);
     c.drop(t);
   }
 }
 
-// InversionAdapter.forward (inversion_adapter.py:22-28): one CLIP ViT-H encoder layer of which only the CLS row is consumed, then
-// LayerNorm + Linear-GELU-Linear-GELU-Linear.  x bf16 [B, T, d]; out bf16 [B, out_dim]
-void adapter_forward(Ctx& c, const T& x /* n=B, h=1, w=T, c=d */, const T& out) {
+// One full pre-LN CLIP encoder layer over all tokens (transformers CLIPEncoderLayer; the sequence of clip.py encoder_layer):
+// LN1 -> fused QKV GEMM -> ladi_attention_small -> out-proj + residual -> LN2 -> fc1 + GELU -> fc2 + residual.  x [B, 1, T, d].
+T adapter_encoder_layer(Ctx& c, const std::string& p, const T& x) {
   const ladi_engine_config& cf = c.e->cfg;
+  const int B = x.n, Tk = x.w, d = x.c, heads = cf.adapter_heads, hd = d / heads;
+  T y = c.layernorm(x.as_rows(), p + "ln1", 1e-5f);
+  ConvOpt oqkv;
+  oqkv.bias = c.F(p + "qkv.b");
+  T qkv = c.gemm(y, c.W(p + "qkv.w"), 3 * d, oqkv);
+  c.drop(y);
+  T a = c.make(B, 1, Tk, d);
+  if (!c.ok()) return a;
+  const long long qbs = (long long)Tk * qkv.pitch, obs = (long long)Tk * a.pitch;
+  const float scale = 1.0f / sqrtf((float)hd);
+  const uint8_t* q = reinterpret_cast<const uint8_t*>(qkv.p);
+  c.rec("attn_small batch=%d heads=%d nq=%d nkv=%d hd=%d q=@%llx qp=%d qbs=%lld k=@%llx kp=%d kbs=%lld v=@%llx vp=%d vbs=%lld out=@%llx op=%d obs=%lld "
+        "scale=%.6g causal=0", B, heads, Tk, Tk, hd, Ctx::A(q), qkv.pitch, qbs, Ctx::A(q + 2 * d), qkv.pitch, qbs, Ctx::A(q + 4 * d), qkv.pitch, qbs,
+        Ctx::A(a.p), a.pitch, obs, (double)scale);
+  if (!c.plan && c.ok()) {
+    const int r = ladi_attention_small(q, q + 2 * d, q + 4 * d, a.p, B, heads, Tk, Tk, hd, qkv.pitch, qkv.pitch, qkv.pitch, a.pitch, qbs, qbs, qbs, obs, scale,
+                                       0, c.st);
+    if (r != LADI_OK) c.rc = r;
+  }
+  c.drop(qkv);
+  ConvOpt oo;
+  oo.bias = c.F(p + "o.b"); oo.residual = &x;
+  T x1 = c.gemm(a, c.W(p + "o.w"), d, oo);
+  c.drop(a);
+  T l2 = c.layernorm(x1, p + "ln2", 1e-5f);
+  ConvOpt o1;
+  o1.bias = c.F(p + "fc1.b"); o1.act = LADI_ACT_GELU;
+  T hmid = c.gemm(l2, c.W(p + "fc1.w"), cf.adapter_mlp, o1);
+  c.drop(l2);
+  ConvOpt o2;
+  o2.bias = c.F(p + "fc2.b"); o2.residual = &x1;
+  T x2 = c.gemm(hmid, c.W(p + "fc2.w"), d, o2);
+  c.drop(hmid); c.drop(x1);
+  return x2.as_image(B, 1, Tk);
+}
+
+// InversionAdapter.forward (inversion_adapter.py:22-28): L CLIP ViT-H encoder layers, then LayerNorm + Linear-GELU-Linear-GELU-Linear
+// on the CLS row.  Layers 0..L-2 (weights `adapter.enc<l>.*`, present only when L > 1) run over all T tokens; of the last layer
+// (weights `adapter.ln1`, `adapter.kv.w`, ...) only the CLS row is consumed, so its query, attention, out-projection and MLP run on one
+// row per image.  x bf16 [B, T, d]; out bf16 [B, out_dim]
+void adapter_forward(Ctx& c, const T& x_in /* n=B, h=1, w=T, c=d */, const T& out) {
+  const ladi_engine_config& cf = c.e->cfg;
+  T xe = x_in;
+  for (int l = 0; c.ok() && c.e->w.count(fmt("adapter.enc%d.ln1.0", l)); ++l) {
+    T nx = adapter_encoder_layer(c, fmt("adapter.enc%d.", l), xe);
+    c.drop(xe);
+    xe = nx;
+  }
+  if (!c.ok()) return;
+  const T& x = xe;
   const int B = x.n, Tk = x.w, d = x.c, heads = cf.adapter_heads, hd = d / heads;
   T y = c.layernorm(x.as_rows(), "adapter.ln1", 1e-5f);
   ConvOpt ok;
@@ -695,7 +761,7 @@ void adapter_forward(Ctx& c, const T& x /* n=B, h=1, w=T, c=d */, const T& out) 
   ConvOpt oo;
   oo.bias = c.F("adapter.o.b"); oo.residual = &x0v;
   T x0 = c.gemm(a, c.W("adapter.o.w"), d, oo);
-  c.drop(a); c.drop(y);
+  c.drop(a); c.drop(y); c.drop(xe);
   T l2 = c.layernorm(x0, "adapter.ln2", 1e-5f);
   ConvOpt o1;
   o1.bias = c.F("adapter.fc1.b"); o1.act = LADI_ACT_GELU;

@@ -34,9 +34,10 @@ def _checkpoint(name, dataset, checkpoint_dir):
     return torch.load(path, map_location="cpu")
 
 
-def inversion_adapter(dataset, checkpoint_dir=None, state_dict=None):
-    """hubconf.py:16-27.  `state_dict=` bypasses the file read (tests, synthetic weights)."""
-    m = InversionAdapter(input_dim=1280, hidden_dim=1280 * 4, output_dim=1024 * 16, num_encoder_layers=1, heads=16, mlp_dim=5120)
+def inversion_adapter(dataset, checkpoint_dir=None, state_dict=None, num_encoder_layers=1):
+    """hubconf.py:16-27.  `state_dict=` bypasses the file read (tests, synthetic weights); `num_encoder_layers` > 1 builds the adapters
+    the training scripts make with `--num_encoder_layers` (the release checkpoints have 1)."""
+    m = InversionAdapter(input_dim=1280, hidden_dim=1280 * 4, output_dim=1024 * 16, num_encoder_layers=num_encoder_layers, heads=16, mlp_dim=5120)
     return m.load_state_dict(state_dict if state_dict is not None else _checkpoint("inversion_adapter", dataset, checkpoint_dir))
 
 
@@ -46,9 +47,10 @@ def extended_unet(dataset, checkpoint_dir=None, state_dict=None):
     return m.load_state_dict(state_dict if state_dict is not None else _checkpoint("unet", dataset, checkpoint_dir))
 
 
-def emasc(dataset, checkpoint_dir=None, state_dict=None):
-    """hubconf.py:40-53."""
-    m = EMASC([128, 128, 128, 256, 512], [128, 256, 512, 512, 512], kernel_size=3, padding=1, stride=1, type="nonlinear")
+def emasc(dataset, checkpoint_dir=None, state_dict=None, kernel_size=3, padding=1, type="nonlinear"):
+    """hubconf.py:40-53 (the release checkpoints are nonlinear 3x3; `kernel_size` / `padding` / `type` select the forms train_emasc.py
+    can make, see vae.EMASC)."""
+    m = EMASC([128, 128, 128, 256, 512], [128, 256, 512, 512, 512], kernel_size=kernel_size, padding=padding, stride=1, type=type)
     return m.load_state_dict(state_dict if state_dict is not None else _checkpoint("emasc", dataset, checkpoint_dir))
 
 

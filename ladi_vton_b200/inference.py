@@ -87,38 +87,46 @@ def check_args(args):
 class SyntheticTryOnDataset(torch.utils.data.Dataset):
     """N samples with the keys, shapes and value ranges the reference datasets return for `outputlist` (src/dataset/vitonhd.py:109-375):
     image / cloth [3,H,W] in [-1,1], im_mask [3,H,W] (the agnostic person image), pose_map [18,H,W] Gaussian heat-maps,
-    inpaint_mask [1,H,W] binary, category str, im_name '<index>.jpg'."""
+    inpaint_mask [1,H,W] binary, category str, im_name '<index>.jpg'; for src/eval.py also warped_cloth [3,H,W] in [-1,1], captions
+    (a noun-chunk string) and clip_cloth_features (fp16 [257, clip_dim], the cache of src/utils/compute_cloth_clip_features.py)."""
 
-    def __init__(self, n, size=(512, 384), categories=('upper_body',), seed=1234):
+    def __init__(self, n, size=(512, 384), categories=('upper_body',), seed=1234, outputlist=None, clip_dim=1280):
         from . import synthetic as S
         self.n, self.size, self.categories = n, size, list(categories)
+        self.outputlist = list(outputlist) if outputlist is not None else OUTPUTLIST
         H, W = size
         self.a = S.synthetic_inputs(n, H, W, seed=seed, ctx_dim=8)
         self.w = S.warp_inputs(n, H, W, seed=seed + 1)
+        if "clip_cloth_features" in self.outputlist:
+            self.clip = torch.randn((n, 257, clip_dim), generator=torch.Generator().manual_seed(seed + 2)).half()
 
     def __len__(self):
         return self.n
 
     def __getitem__(self, i):
         mask = self.a["mask_image"][i]
-        return dict(image=self.a["image"][i], cloth=self.w["cloth"][i], im_mask=self.a["image"][i] * (mask < 0.5), pose_map=self.a["pose_map"][i],
-                    inpaint_mask=mask, category=self.categories[i % len(self.categories)], im_name=f"{i:05d}_00.jpg")
+        cat = self.categories[i % len(self.categories)]
+        get = dict(image=lambda: self.a["image"][i], cloth=lambda: self.w["cloth"][i], im_mask=lambda: self.a["image"][i] * (mask < 0.5),
+                   pose_map=lambda: self.a["pose_map"][i], inpaint_mask=lambda: mask, category=lambda: cat, im_name=lambda: f"{i:05d}_00.jpg",
+                   warped_cloth=lambda: self.a["warped_cloth"][i], captions=lambda: f"{CATEGORY_TEXT[cat].split(' ', 1)[1]}, sample {i}",
+                   clip_cloth_features=lambda: self.clip[i])
+        return {k: get[k]() for k in self.outputlist}
 
 
-def build_dataset(args, category):
-    """src/inference.py:149-180."""
+def build_dataset(args, category, outputlist=OUTPUTLIST):
+    """src/inference.py:149-180 (src/eval.py:289-310 with its own `outputlist`)."""
     if args.synthetic_samples > 0:
         cats = category if args.dataset == "dresscode" else ['upper_body']
-        return SyntheticTryOnDataset(args.synthetic_samples, (512, 384), cats, args.seed)
+        return SyntheticTryOnDataset(args.synthetic_samples, (512, 384), cats, args.seed, outputlist)
     if args.reference_src and args.reference_src not in sys.path:
         sys.path.insert(0, args.reference_src)
     try:
         if args.dataset == "dresscode":
             from dataset.dresscode import DressCodeDataset
             return DressCodeDataset(dataroot_path=args.dresscode_dataroot, phase='test', order=args.test_order, radius=5,
-                                    outputlist=OUTPUTLIST, category=category, size=(512, 384))
+                                    outputlist=outputlist, category=category, size=(512, 384))
         from dataset.vitonhd import VitonHDDataset
-        return VitonHDDataset(dataroot_path=args.vitonhd_dataroot, phase='test', order=args.test_order, radius=5, outputlist=OUTPUTLIST,
+        return VitonHDDataset(dataroot_path=args.vitonhd_dataroot, phase='test', order=args.test_order, radius=5, outputlist=outputlist,
                               size=(512, 384))
     except ImportError as e:
         raise ImportError("the dataset classes are the reference's own (src/dataset/*.py, out of this engine's scope): pass "

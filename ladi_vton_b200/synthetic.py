@@ -17,11 +17,16 @@ def emasc_channels(vae_ch):
     return [c[0], c[0], c[0], c[1], c[2]], [c[0], c[1], c[2], c[3], c[3]]
 
 
-def emasc_param_shapes(cin, cout):
+def emasc_param_shapes(cin, cout, kernel_size=3, type="nonlinear"):
+    """State-dict shapes of src/models/emasc.py's EMASC (the linear form is always 3x3, emasc.py:21-24)."""
     S = {}
     for i, (a, b) in enumerate(zip(cin, cout)):
-        S[f"conv.{i}.0.weight"], S[f"conv.{i}.0.bias"] = (a, a, 3, 3), (a,)
-        S[f"conv.{i}.2.weight"], S[f"conv.{i}.2.bias"] = (b, a, 3, 3), (b,)
+        if type == "linear":
+            S[f"conv.{i}.weight"], S[f"conv.{i}.bias"] = (b, a, 3, 3), (b,)
+            continue
+        k = kernel_size
+        S[f"conv.{i}.0.weight"], S[f"conv.{i}.0.bias"] = (a, a, k, k), (a,)
+        S[f"conv.{i}.2.weight"], S[f"conv.{i}.2.bias"] = (b, a, k, k), (b,)
     return S
 
 

@@ -343,11 +343,24 @@ class AutoencoderKL:
 
 
 class EMASC:
-    """emasc.py:11-40 ('nonlinear'): per scale Conv3x3 -> SiLU -> Conv3x3; state-dict keys conv.{i}.{0,2}.{weight,bias}."""
+    """emasc.py:11-40: per scale either the nonlinear form Conv(k) -> SiLU -> Conv(k) (state-dict keys conv.{i}.{0,2}.{weight,bias}; the
+    hub checkpoints are k = 3) or the linear form, one Conv3x3 (keys conv.{i}.{weight,bias}; the reference's linear EMASC always builds a
+    3x3 kernel and ignores `kernel_size`, emasc.py:21-24).  `mask_features` is folded into the last conv's epilogue."""
 
     def __init__(self, in_channels, out_channels, kernel_size=3, padding=1, stride=1, type="nonlinear"):
-        if type != "nonlinear" or kernel_size != 3 or padding != 1 or stride != 1:
-            raise NotImplementedError("only the nonlinear 3x3 EMASC of hubconf.py:40-53 is implemented")
+        if type not in ("linear", "nonlinear"):
+            raise NotImplementedError(f"EMASC type {type} is not implemented.")
+        k = 3 if type == "linear" else int(kernel_size)
+        if stride != 1 or k % 2 == 0 or padding != (k - 1) // 2:
+            raise NotImplementedError(
+                f"EMASC with kernel {k}, padding {padding}, stride {stride} is not built: the output must keep the feature's resolution "
+                "(a 'same' convolution), otherwise the decoder's skip add `sample += int_feat` (src/models/vae.py:193) fails in the "
+                "reference itself")
+        if k not in (1, 3):
+            raise NotImplementedError(
+                f"EMASC with a {k}x{k} kernel is not built: {k * k} taps exceed the 24 K segments (MAX_SEG) of the convolution kernel "
+                "(csrc/convgemm.cu); only 3x3 and 1x1 EMASC run on it")
+        self.type, self.kernel_size, self.padding = type, k, padding
         self.in_channels, self.out_channels = list(in_channels), list(out_channels)
         self.device = torch.device("cpu")
         self._sd, self.P = None, None
@@ -359,10 +372,15 @@ class EMASC:
     def requires_grad_(self, flag=False):
         return self
 
+    def param_shapes(self):
+        from .synthetic import emasc_param_shapes
+        return emasc_param_shapes(self.in_channels, self.out_channels, self.kernel_size, self.type)
+
     def load_state_dict(self, sd, strict=True):
-        want = {f"conv.{i}.{j}.{n}" for i in range(len(self.in_channels)) for j in (0, 2) for n in ("weight", "bias")}
-        if strict and set(sd.keys()) != want:
-            raise RuntimeError(f"EMASC state_dict mismatch: {sorted(set(sd.keys()) ^ want)[:6]}")
+        want = self.param_shapes()
+        bad = sorted(set(sd.keys()) ^ set(want)) + [k for k in want if k in sd and tuple(sd[k].shape) != tuple(want[k])]
+        if strict and bad:
+            raise RuntimeError(f"EMASC state_dict mismatch: {bad[:6]}")
         self._sd = {k: v.detach() for k, v in sd.items()}
         if self.device.type == "cuda":
             self._pack()
@@ -385,17 +403,26 @@ class EMASC:
     def _pack(self):
         g = lambda k: self._sd[k].to(self.device, torch.float32)
         self.P = []
-        for i, (ci, co) in enumerate(zip(self.in_channels, self.out_channels)):
-            self.P.append((pack_conv(g(f"conv.{i}.0.weight"), [ci]), f32(g(f"conv.{i}.0.bias")),
-                           pack_conv(g(f"conv.{i}.2.weight"), [ci]), f32(g(f"conv.{i}.2.bias"))))
+        for i, ci in enumerate(self.in_channels):
+            if self.type == "linear":  # (w, b)
+                self.P.append((pack_conv(g(f"conv.{i}.weight"), [ci]), f32(g(f"conv.{i}.bias"))))
+            else:  # (w1, b1, w2, b2)
+                self.P.append((pack_conv(g(f"conv.{i}.0.weight"), [ci]), f32(g(f"conv.{i}.0.bias")),
+                               pack_conv(g(f"conv.{i}.2.weight"), [ci]), f32(g(f"conv.{i}.2.bias"))))
         self.pack_gen += 1
         self.engine = None
         if eng.enabled() and self.device.type == "cuda":
-            W = {}
-            for i, (w1, b1, w2, b2) in enumerate(self.P):
-                W.update({f"emasc.{i}.w1": w1, f"emasc.{i}.b1": b1, f"emasc.{i}.w2": w2, f"emasc.{i}.b2": b2})
-            self._engine_weights = W
+            self._engine_weights = self.engine_weights()
             self.engine = {}  # one handle per resolution pyramid (the strides are part of the handle's config), built on first use
+
+    def engine_weights(self):
+        """Weight table of ladi_emasc_forward: emasc.<i>.w1/b1 (+ w2/b2 for the nonlinear form; the engine reads the form and the kernel
+        size from the table, include/ladi_b200.h)."""
+        W = {}
+        for i, t in enumerate(self.P):
+            for name, v in zip(("w1", "b1", "w2", "b2"), t):
+                W[f"emasc.{i}.{name}"] = v
+        return W
 
     def _engine_for(self, feats):
         H, Wd = feats[0].shape[1], feats[0].shape[2]
@@ -420,8 +447,14 @@ class EMASC:
             lib.call("ladi_emasc_forward", e.h, eng.ptr_array(feats), inv, B, H, Wd, eng.ptr_array(outs), ops._ptr(ws), ws.numel(), ops._stream())
             return outs
         out = []
+        k, p = self.kernel_size, self.padding
         for i, f in enumerate(feats):
+            rs = None if inv_masks is None else inv_masks[i]
+            if self.type == "linear":
+                w, b = self.P[i]
+                out.append(ops.conv2d([f], w, self.out_channels[i], ksize=k, pad_lo=p, bias=b, row_scale=rs))
+                continue
             w1, b1, w2, b2 = self.P[i]
-            t = ops.conv2d([f], w1, self.in_channels[i], bias=b1, act=ops.ACT_SILU)
-            out.append(ops.conv2d([t], w2, self.out_channels[i], bias=b2, row_scale=None if inv_masks is None else inv_masks[i]))
+            t = ops.conv2d([f], w1, self.in_channels[i], ksize=k, pad_lo=p, bias=b1, act=ops.ACT_SILU)
+            out.append(ops.conv2d([t], w2, self.out_channels[i], ksize=k, pad_lo=p, bias=b2, row_scale=rs))
         return out
