@@ -1,0 +1,335 @@
+// Kernels of the image-quality metrics (ladi_vton_b200/metrics.py, the engine form of the reference's src/utils/val_metrics.py):
+// the im2col / pooling glue of the FID Inception-v3 and of the LPIPS AlexNet (their convolutions run on the wgmma GEMM, convgemm.cu),
+// the LPIPS distance layer, SSIM, and torch-fidelity's TF1-style bilinear resize for the Inception Score.  Every reduction has a fixed
+// order (no floating-point atomics), so two runs give identical bits.
+#include "common.h"
+#include "ptx.cuh"
+
+namespace {
+
+inline int grid_for(long long total) {
+  long long g = (total + 255) / 256;
+  const long long cap = (long long)ladi_num_sms() * 16;
+  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
+}
+
+// NHWC bf16 [n,h,w,pitch] -> rows [n*oh*ow, k_pad], column (ky*kw + kx)*c + ch, 8 channels (16 bytes) per thread; c % 8 == 0.
+__global__ void __launch_bounds__(256) im2col_nhwc_kernel(const bf16* __restrict__ x, int h, int w, int c, int pitch, int kh, int kw, int sh,
+                                                          int sw, int ph, int pw, int oh, int ow, long long rows, bf16* __restrict__ out,
+                                                          int k_pad) {
+  ptx::pdl_wait();
+  const int groups = k_pad >> 3, k_true = kh * kw * c;
+  const long long total = rows * groups;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const int col = (int)(i % groups) * 8;
+    const long long r = i / groups;
+    uint4 v = make_uint4(0u, 0u, 0u, 0u);
+    if (col < k_true) {
+      const int tap = col / c, ch = col - tap * c, ky = tap / kw, kx = tap - ky * kw;
+      const int ox = (int)(r % ow), oy = (int)((r / ow) % oh);
+      const long long b = r / ((long long)ow * oh);
+      const int iy = oy * sh - ph + ky, ix = ox * sw - pw + kx;
+      if (iy >= 0 && iy < h && ix >= 0 && ix < w)
+        v = __ldg(reinterpret_cast<const uint4*>(x + ((b * h + iy) * w + ix) * pitch + ch));
+    }
+    *reinterpret_cast<uint4*>(out + r * k_pad + col) = v;
+  }
+}
+
+// NCHW fp32 pixels -> the same rows; (x - shift[ch]) / scale[ch] is applied to in-image pixels BEFORE the zero padding.
+__global__ void __launch_bounds__(256) im2col_pixels_kernel(const float* __restrict__ x, int c, int h, int w, int kh, int kw, int sh, int sw,
+                                                            int ph, int pw, int oh, int ow, long long rows, const float* __restrict__ shift,
+                                                            const float* __restrict__ scale, bf16* __restrict__ out, int k_pad) {
+  ptx::pdl_wait();
+  const int k_true = kh * kw * c;
+  const long long total = rows * k_pad;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const int col = (int)(i % k_pad);
+    const long long r = i / k_pad;
+    float v = 0.f;
+    if (col < k_true) {
+      const int tap = col / c, ch = col - tap * c, ky = tap / kw, kx = tap - ky * kw;
+      const int ox = (int)(r % ow), oy = (int)((r / ow) % oh);
+      const long long b = r / ((long long)ow * oh);
+      const int iy = oy * sh - ph + ky, ix = ox * sw - pw + kx;
+      if (iy >= 0 && iy < h && ix >= 0 && ix < w) v = (__ldg(x + ((b * c + ch) * h + iy) * w + ix) - __ldg(shift + ch)) / __ldg(scale + ch);
+    }
+    out[i] = __float2bfloat16(v);
+  }
+}
+
+// torch max_pool2d / avg_pool2d (ceil_mode=False) on NHWC bf16, 8 channels per thread, output into channels [c_off, c_off + c) of
+// `out` [n, oh, ow, out_pitch].  Average: fp32 sum in window order, divided by the window size counted as torch does.
+__global__ void __launch_bounds__(256) pool2d_kernel(const bf16* __restrict__ x, int h, int w, int c, int pitch, int k, int s, int p, int mode,
+                                                     int oh, int ow, long long pixels, bf16* __restrict__ out, int out_pitch, int c_off) {
+  ptx::pdl_wait();
+  const int nv = c >> 3;
+  const long long total = pixels * nv;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const int v = (int)(i % nv);
+    const long long px = i / nv;
+    const int ox = (int)(px % ow), oy = (int)((px / ow) % oh);
+    const long long b = px / ((long long)ow * oh);
+    int y0 = oy * s - p, x0 = ox * s - p;
+    int y1 = min(y0 + k, h + p), x1 = min(x0 + k, w + p);
+    const int padded = (y1 - y0) * (x1 - x0);
+    y0 = max(y0, 0); x0 = max(x0, 0); y1 = min(y1, h); x1 = min(x1, w);
+    float acc[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[j] = mode == LADI_POOL_MAX ? -INFINITY : 0.f;
+    for (int yy = y0; yy < y1; ++yy)
+      for (int xx = x0; xx < x1; ++xx) {
+        const uint4 u = __ldg(reinterpret_cast<const uint4*>(x + ((b * h + yy) * w + xx) * pitch + v * 8));
+        const float f[8] = {ptx::bf16_lo(u.x), ptx::bf16_hi(u.x), ptx::bf16_lo(u.y), ptx::bf16_hi(u.y),
+                            ptx::bf16_lo(u.z), ptx::bf16_hi(u.z), ptx::bf16_lo(u.w), ptx::bf16_hi(u.w)};
+#pragma unroll
+        for (int j = 0; j < 8; ++j) acc[j] = mode == LADI_POOL_MAX ? fmaxf(acc[j], f[j]) : acc[j] + f[j];
+      }
+    if (mode != LADI_POOL_MAX) {
+      const float inv = 1.f / (float)(mode == LADI_POOL_AVG ? padded : (y1 - y0) * (x1 - x0));
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc[j] *= inv;
+    }
+    uint4 r;
+    r.x = ptx::pack_bf16(acc[0], acc[1]); r.y = ptx::pack_bf16(acc[2], acc[3]);
+    r.z = ptx::pack_bf16(acc[4], acc[5]); r.w = ptx::pack_bf16(acc[6], acc[7]);
+    *reinterpret_cast<uint4*>(out + px * out_pitch + c_off + v * 8) = r;
+  }
+}
+
+// adaptive_avg_pool2d(x, 1).flatten(1): out fp32 [n, out_pitch], one thread per (image, channel), pixels summed in order.
+__global__ void __launch_bounds__(256) global_avg_kernel(const bf16* __restrict__ x, int n, int hw, int c, int pitch, float* __restrict__ out,
+                                                         int out_pitch) {
+  ptx::pdl_wait();
+  const long long total = (long long)n * c;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const int ch = (int)(i % c);
+    const long long b = i / c;
+    const bf16* p = x + b * hw * pitch + ch;
+    float acc = 0.f;
+    for (int q = 0; q < hw; ++q) acc += __bfloat162float(p[(long long)q * pitch]);
+    out[b * out_pitch + ch] = acc / (float)hw;
+  }
+}
+
+// One LPIPS layer (lpips.LPIPS.forward, version 0.1): per pixel na = a / (|a| + 1e-10), nb likewise, d = sum_c lin[c] (na - nb)^2;
+// acc[b] += mean over pixels of d.  One block per image; warp w takes pixels w, w + 16, ...; warps combined in index order.
+constexpr int LPIPS_WARPS = 16;
+__global__ void __launch_bounds__(LPIPS_WARPS * 32) lpips_layer_kernel(const bf16* __restrict__ fa, const bf16* __restrict__ fb, int hw, int c,
+                                                                       int pitch, const float* __restrict__ lin, float* __restrict__ acc) {
+  ptx::pdl_wait();
+  __shared__ float part[LPIPS_WARPS];
+  const int b = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const bf16* A = fa + (long long)b * hw * pitch;
+  const bf16* B = fb + (long long)b * hw * pitch;
+  float mine = 0.f;
+  for (int q = warp; q < hw; q += LPIPS_WARPS) {
+    const bf16* pa = A + (long long)q * pitch;
+    const bf16* pb = B + (long long)q * pitch;
+    float sa = 0.f, sb = 0.f;
+    for (int ch = lane; ch < c; ch += 32) {
+      const float a = __bfloat162float(pa[ch]), bb = __bfloat162float(pb[ch]);
+      sa = fmaf(a, a, sa);
+      sb = fmaf(bb, bb, sb);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      sa += __shfl_xor_sync(0xffffffffu, sa, o);
+      sb += __shfl_xor_sync(0xffffffffu, sb, o);
+    }
+    const float ra = 1.f / (sqrtf(sa) + 1e-10f), rb = 1.f / (sqrtf(sb) + 1e-10f);
+    float d = 0.f;
+    for (int ch = lane; ch < c; ch += 32) {
+      const float t = __bfloat162float(pa[ch]) * ra - __bfloat162float(pb[ch]) * rb;
+      d = fmaf(__ldg(lin + ch), t * t, d);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+    mine += d;
+  }
+  if (lane == 0) part[warp] = mine;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float t = 0.f;
+    for (int i = 0; i < LPIPS_WARPS; ++i) t += part[i];
+    acc[b] += t / (float)hw;
+  }
+}
+
+// SSIM (torchmetrics StructuralSimilarityIndexMeasure, gaussian 11 x 11, sigma 1.5): one 16 x 16 tile of valid positions (window fully
+// inside the image) per block, all channels; separable filtering through shared memory; the block's sum goes to partial[b][tile].
+constexpr int SSIM_T = 16, SSIM_K = 11, SSIM_S = SSIM_T + SSIM_K - 1;
+__global__ void __launch_bounds__(SSIM_T * SSIM_T) ssim_tile_kernel(const float* __restrict__ x, const float* __restrict__ y, int c, int h, int w,
+                                                                    float* __restrict__ partial) {
+  ptx::pdl_wait();
+  __shared__ float g[SSIM_K];
+  __shared__ float sx[SSIM_S][SSIM_S], sy[SSIM_S][SSIM_S];
+  __shared__ float hs[5][SSIM_S][SSIM_T];
+  __shared__ float red[SSIM_T * SSIM_T];
+  const int tx = threadIdx.x, ty = threadIdx.y, t = ty * SSIM_T + tx;
+  const int b = blockIdx.z, x0 = blockIdx.x * SSIM_T, y0 = blockIdx.y * SSIM_T;
+  const int vh = h - SSIM_K + 1, vw = w - SSIM_K + 1;
+  if (t == 0) {
+    float s = 0.f;
+    for (int k = 0; k < SSIM_K; ++k) {
+      const float d = ((float)k - 5.f) / 1.5f;
+      g[k] = expf(-0.5f * d * d);
+      s += g[k];
+    }
+    for (int k = 0; k < SSIM_K; ++k) g[k] /= s;
+  }
+  const float C1 = 0.01f * 0.01f, C2 = 0.03f * 0.03f;
+  float mine = 0.f;
+  for (int ch = 0; ch < c; ++ch) {
+    __syncthreads();
+    const float* X = x + ((long long)b * c + ch) * h * w;
+    const float* Y = y + ((long long)b * c + ch) * h * w;
+    for (int i = t; i < SSIM_S * SSIM_S; i += SSIM_T * SSIM_T) {
+      const int r = i / SSIM_S, q = i - r * SSIM_S, gy = y0 + r, gx = x0 + q;
+      const bool in = gy < h && gx < w;
+      sx[r][q] = in ? __ldg(X + (long long)gy * w + gx) : 0.f;
+      sy[r][q] = in ? __ldg(Y + (long long)gy * w + gx) : 0.f;
+    }
+    __syncthreads();
+    for (int r = ty; r < SSIM_S; r += SSIM_T) {
+      float m0 = 0.f, m1 = 0.f, m2 = 0.f, m3 = 0.f, m4 = 0.f;
+#pragma unroll
+      for (int k = 0; k < SSIM_K; ++k) {
+        const float a = sx[r][tx + k], bb = sy[r][tx + k], gk = g[k];
+        m0 = fmaf(gk, a, m0);
+        m1 = fmaf(gk, bb, m1);
+        m2 = fmaf(gk, a * a, m2);
+        m3 = fmaf(gk, bb * bb, m3);
+        m4 = fmaf(gk, a * bb, m4);
+      }
+      hs[0][r][tx] = m0; hs[1][r][tx] = m1; hs[2][r][tx] = m2; hs[3][r][tx] = m3; hs[4][r][tx] = m4;
+    }
+    __syncthreads();
+    if (y0 + ty < vh && x0 + tx < vw) {
+      float m[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+      for (int k = 0; k < SSIM_K; ++k)
+#pragma unroll
+        for (int q = 0; q < 5; ++q) m[q] = fmaf(g[k], hs[q][ty + k][tx], m[q]);
+      const float mxx = m[0] * m[0], myy = m[1] * m[1], mxy = m[0] * m[1];
+      const float vx = m[2] - mxx, vy = m[3] - myy, cxy = m[4] - mxy;
+      mine += ((2.f * mxy + C1) * (2.f * cxy + C2)) / ((mxx + myy + C1) * (vx + vy + C2));
+    }
+  }
+  red[t] = mine;
+  __syncthreads();
+  for (int o = SSIM_T * SSIM_T / 2; o > 0; o >>= 1) {
+    if (t < o) red[t] += red[t + o];
+    __syncthreads();
+  }
+  if (t == 0) partial[(long long)b * gridDim.x * gridDim.y + blockIdx.y * gridDim.x + blockIdx.x] = red[0];
+}
+
+// second pass: out[b] = (sum of the image's tile partials, fixed tree order) / (c * valid positions)
+__global__ void __launch_bounds__(256) ssim_reduce_kernel(const float* __restrict__ partial, int tiles, float inv_count, float* __restrict__ out) {
+  ptx::pdl_wait();
+  __shared__ float red[256];
+  const int b = blockIdx.x, t = threadIdx.x;
+  float s = 0.f;
+  for (int i = t; i < tiles; i += 256) s += partial[(long long)b * tiles + i];
+  red[t] = s;
+  __syncthreads();
+  for (int o = 128; o > 0; o >>= 1) {
+    if (t < o) red[t] += red[t + o];
+    __syncthreads();
+  }
+  if (t == 0) out[b] = red[0] * inv_count;
+}
+
+// torch-fidelity's TF1 bilinear resize of (x * 255).byte() (torchmetrics InceptionScore, normalize=True): source coordinate
+// o * (in / out) with no half-pixel offset, upper neighbour clamped to the edge; NCHW fp32 in [0, 1] -> NCHW fp32 in [0, 255].
+__global__ void __launch_bounds__(256) resize_tf1_kernel(const float* __restrict__ x, int h, int w, int oh, int ow, long long planes,
+                                                         float* __restrict__ out) {
+  ptx::pdl_wait();
+  const float sy = (float)h / (float)oh, sx = (float)w / (float)ow;
+  const long long total = planes * oh * ow;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
+    const int ox = (int)(i % ow), oy = (int)((i / ow) % oh);
+    const long long pl = i / ((long long)ow * oh);
+    const float fy = (float)oy * sy, fx = (float)ox * sx;
+    const int iy0 = min((int)floorf(fy), h - 1), ix0 = min((int)floorf(fx), w - 1);
+    const int iy1 = min(iy0 + 1, h - 1), ix1 = min(ix0 + 1, w - 1);
+    const float ly = fy - (float)iy0, lx = fx - (float)ix0;
+    const float* P = x + pl * h * w;
+    auto px = [&](int yy, int xx) { return truncf(fminf(fmaxf(__fmul_rn(__ldg(P + (long long)yy * w + xx), 255.f), 0.f), 255.f)); };
+    const float tl = px(iy0, ix0), tr = px(iy0, ix1), bl = px(iy1, ix0), br = px(iy1, ix1);
+    const float top = tl + (tr - tl) * lx, bot = bl + (br - bl) * lx;
+    out[i] = top + (bot - top) * ly;
+  }
+}
+
+}  // namespace
+
+#define STREAM reinterpret_cast<cudaStream_t>(stream)
+
+extern "C" int ladi_im2col_bf16(const void* x, int x_is_f32_nchw, int n, int c, int h, int w, int pitch, int kh, int kw, int sh, int sw, int ph,
+                                int pw, const float* shift, const float* scale, void* out, int k_pad, void* stream) {
+  LADI_CHECK(x && out && n > 0 && c > 0 && h > 0 && w > 0 && kh > 0 && kw > 0 && sh > 0 && sw > 0 && ph >= 0 && pw >= 0, "im2col: bad extent");
+  const int oh = (h + 2 * ph - kh) / sh + 1, ow = (w + 2 * pw - kw) / sw + 1;
+  LADI_CHECK(h + 2 * ph >= kh && w + 2 * pw >= kw && oh > 0 && ow > 0, "im2col: window larger than the padded image");
+  LADI_CHECK(k_pad % 8 == 0 && k_pad >= kh * kw * c, "im2col: k_pad must be a multiple of 8 and >= kh*kw*c");
+  const long long rows = (long long)n * oh * ow;
+  if (x_is_f32_nchw) {
+    LADI_CHECK(shift && scale, "im2col: the pixel form needs shift and scale");
+    LADI_CUDA(ladi_launch(im2col_pixels_kernel, dim3(grid_for(rows * k_pad)), dim3(256), 0, STREAM, (const float*)x, c, h, w, kh, kw, sh, sw, ph,
+                          pw, oh, ow, rows, shift, scale, (bf16*)out, k_pad));
+  } else {
+    LADI_CHECK(!shift && !scale, "im2col: shift / scale apply to the fp32 pixel form only");
+    LADI_CHECK(c % 8 == 0 && pitch % 8 == 0 && pitch >= c, "im2col: C and pitch must be multiples of 8");
+    LADI_CUDA(ladi_launch(im2col_nhwc_kernel, dim3(grid_for(rows * (k_pad / 8))), dim3(256), 0, STREAM, (const bf16*)x, h, w, c, pitch, kh, kw, sh,
+                          sw, ph, pw, oh, ow, rows, (bf16*)out, k_pad));
+  }
+  return LADI_OK;
+}
+
+extern "C" int ladi_pool2d_bf16(const void* x, int n, int h, int w, int c, int x_pitch, int k, int s, int p, int mode, void* out, int out_pitch,
+                                int c_off, void* stream) {
+  LADI_CHECK(x && out && n > 0 && h > 0 && w > 0 && c > 0, "pool2d: bad extent");
+  LADI_CHECK(c % 8 == 0 && x_pitch % 8 == 0 && x_pitch >= c, "pool2d: C and pitch must be multiples of 8");
+  if (mode == LADI_POOL_GLOBAL_AVG_F32) {
+    LADI_CHECK(out_pitch >= c_off + c, "pool2d: channel window outside the output pitch");
+    LADI_CUDA(ladi_launch(global_avg_kernel, dim3(grid_for((long long)n * c)), dim3(256), 0, STREAM, (const bf16*)x, n, h * w, c, x_pitch,
+                          (float*)out + c_off, out_pitch));
+    return LADI_OK;
+  }
+  LADI_CHECK(mode == LADI_POOL_MAX || mode == LADI_POOL_AVG || mode == LADI_POOL_AVG_EXCLUDE_PAD, "pool2d: unknown mode %d", mode);
+  LADI_CHECK(k > 0 && s > 0 && p >= 0 && 2 * p <= k && h + 2 * p >= k && w + 2 * p >= k, "pool2d: bad window (k %d, s %d, p %d)", k, s, p);
+  LADI_CHECK(out_pitch % 8 == 0 && c_off % 8 == 0 && out_pitch >= c_off + c, "pool2d: output pitch / channel offset must be multiples of 8");
+  const int oh = (h + 2 * p - k) / s + 1, ow = (w + 2 * p - k) / s + 1;
+  const long long pixels = (long long)n * oh * ow;
+  LADI_CUDA(ladi_launch(pool2d_kernel, dim3(grid_for(pixels * (c / 8))), dim3(256), 0, STREAM, (const bf16*)x, h, w, c, x_pitch, k, s, p, mode, oh,
+                        ow, pixels, (bf16*)out, out_pitch, c_off));
+  return LADI_OK;
+}
+
+extern "C" int ladi_lpips_layer(const void* fa, const void* fb, int n, int h, int w, int c, int pitch, const float* lin, float* acc, void* stream) {
+  LADI_CHECK(fa && fb && lin && acc && n > 0 && h > 0 && w > 0 && c > 0 && pitch >= c, "lpips_layer: bad extent");
+  LADI_CUDA(ladi_launch(lpips_layer_kernel, dim3(n), dim3(LPIPS_WARPS * 32), 0, STREAM, (const bf16*)fa, (const bf16*)fb, h * w, c, pitch, lin, acc));
+  return LADI_OK;
+}
+
+extern "C" int ladi_ssim_partials(int h, int w) {
+  if (h < SSIM_K || w < SSIM_K) return -1;
+  return ((h - SSIM_K + 1 + SSIM_T - 1) / SSIM_T) * ((w - SSIM_K + 1 + SSIM_T - 1) / SSIM_T);
+}
+
+extern "C" int ladi_ssim_f32(const float* x, const float* y, int n, int c, int h, int w, float* ws, float* out, void* stream) {
+  LADI_CHECK(x && y && ws && out && n > 0 && c > 0, "ssim: bad arguments");
+  LADI_CHECK(h >= SSIM_K && w >= SSIM_K, "ssim: images must be at least 11 x 11 (got %d x %d)", h, w);
+  const dim3 grid((w - SSIM_K + 1 + SSIM_T - 1) / SSIM_T, (h - SSIM_K + 1 + SSIM_T - 1) / SSIM_T, n);
+  LADI_CUDA(ladi_launch(ssim_tile_kernel, grid, dim3(SSIM_T, SSIM_T), 0, STREAM, x, y, c, h, w, ws));
+  const float inv = (float)(1.0 / ((double)c * (h - SSIM_K + 1) * (w - SSIM_K + 1)));
+  LADI_CUDA(ladi_launch(ssim_reduce_kernel, dim3(n), dim3(256), 0, STREAM, (const float*)ws, (int)(grid.x * grid.y), inv, out));
+  return LADI_OK;
+}
+
+extern "C" int ladi_resize_tf1_u8(const float* x, int n, int c, int h, int w, int oh, int ow, float* out, void* stream) {
+  LADI_CHECK(x && out && n > 0 && c > 0 && h > 0 && w > 0 && oh > 0 && ow > 0, "resize_tf1: bad extent");
+  LADI_CUDA(ladi_launch(resize_tf1_kernel, dim3(grid_for((long long)n * c * oh * ow)), dim3(256), 0, STREAM, x, h, w, oh, ow, (long long)n * c, out));
+  return LADI_OK;
+}

@@ -21,6 +21,8 @@ What differs, because the target boxes have no network (the reference downloads 
     writes;
   * `--allow_tf32`, `--enable_xformers_memory_efficient_attention` are accepted: the engine always computes in bf16 and its attention is
     already fused.
+Scoring on the engine (instead of `--compute_metrics`, which runs the reference's own val_metrics.py from `--reference_src`):
+`python -m ladi_vton_b200.val_metrics --gen_folder <output_dir>/<save_name>_<test_order> --test_order <order> --dataset ... --metrics_weights_dir W`.
 """
 import argparse
 import json

@@ -18,6 +18,8 @@ What differs, because the target boxes have no network (the reference downloads 
     LOCAL_RANK is set, :91-93; here LOCAL_RANK just selects the device.)
   * `--mixed_precision`, `--allow_tf32`, `--enable_xformers_memory_efficient_attention` are accepted: the engine always computes in bf16
     with fp32 accumulation and its attention is already fused.
+  * `--compute_metrics` runs the reference's own src/utils/val_metrics.py from `--reference_src`; to score the written images on the
+    engine instead: `python -m ladi_vton_b200.val_metrics --gen_folder <output_dir> --test_order <order> --dataset ... --metrics_weights_dir W`.
 """
 import argparse
 import json

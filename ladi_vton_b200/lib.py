@@ -98,6 +98,13 @@ SIGNATURES = {
     "ladi_maxpool2_nhwc": ([_P, _I, _I, _I, _I, _P, _P], _I),
     "ladi_upsample2x_bilinear_ac": ([_P, _I, _I, _I, _I, _P, _P], _I),
     "ladi_nhwc_f32_to_nchw_clamp": ([_P, _I, _I, _I, _I, _I, _F, _F, _P, _P], _I),
+    # ---- image-quality metrics (csrc/metrics.cu)
+    "ladi_im2col_bf16": ([_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _I, _P], _I),
+    "ladi_pool2d_bf16": ([_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _I, _I, _P], _I),
+    "ladi_lpips_layer": ([_P, _P, _I, _I, _I, _I, _I, _P, _P, _P], _I),
+    "ladi_ssim_partials": ([_I, _I], _I),
+    "ladi_ssim_f32": ([_P, _P, _I, _I, _I, _I, _P, _P, _P], _I),
+    "ladi_resize_tf1_u8": ([_P, _I, _I, _I, _I, _I, _I, _P, _P], _I),
     # ---- module-level ABI (csrc/engine.cu)
     "ladi_engine_create": ([C.POINTER(EngineConfig), C.POINTER(Weight), _I, _PP], _I),
     "ladi_engine_destroy": ([_P], _I),

@@ -500,3 +500,81 @@ def nhwc_f32_to_nchw_clamp(x, c, lo, hi):
     out = torch.empty((n, c, h, w), dtype=torch.float32, device=x.device)
     _call("ladi_nhwc_f32_to_nchw_clamp", 0.0, _ptr(x), n, c, h, w, pitch, float(lo), float(hi), _ptr(out), _stream())
     return out
+
+
+# ---- image-quality metrics (csrc/metrics.cu) ------------------------------------------------------------------------------------------
+POOL_MAX, POOL_AVG, POOL_AVG_EXCLUDE_PAD, POOL_GLOBAL_AVG_F32 = 0, 1, 2, 3
+
+
+def conv_out_size(size, k, s, p):
+    return (size + 2 * p - k) // s + 1
+
+
+def im2col(x, kernel, stride, padding, k_pad, shift=None, scale=None):
+    """Rows [n*oh*ow, k_pad] bf16, column (ky*kw + kx)*c + ch, of a kernel=(kh, kw) / stride=(sh, sw) / padding=(ph, pw) convolution.
+    x: NHWC bf16 (channel-sliced views fine, c % 8 == 0), or NCHW fp32 pixels with per-channel fp32 `shift` / `scale` applied as
+    (x - shift) / scale before the zero padding."""
+    (kh, kw), (sh, sw), (ph, pw) = kernel, stride, padding
+    pixels = x.dtype == torch.float32
+    if pixels:
+        assert x.is_contiguous() and shift is not None and scale is not None
+        n, c, h, w = x.shape
+        pitch = 0
+    else:
+        assert x.dtype == torch.bfloat16 and shift is None and scale is None
+        n, h, w, c, pitch = _nhwc(x)
+    oh, ow = conv_out_size(h, kh, sh, ph), conv_out_size(w, kw, sw, pw)
+    out = torch.empty((n * oh * ow, k_pad), dtype=torch.bfloat16, device=x.device)
+    _call("ladi_im2col_bf16", 0.0, _ptr(x), int(pixels), n, c, h, w, pitch, kh, kw, sh, sw, ph, pw, _ptr(shift), _ptr(scale), _ptr(out), k_pad,
+          _stream())
+    return out, (n, oh, ow)
+
+
+def pool2d(x, k, s, p, mode, out=None, c_off=0):
+    """torch max_pool2d / avg_pool2d on NHWC bf16; the result goes to channels [c_off, c_off + C) of `out` when given."""
+    n, h, w, c, pitch = _nhwc(x)
+    oh, ow = conv_out_size(h, k, s, p), conv_out_size(w, k, s, p)
+    if out is None:
+        out = torch.empty((n, oh, ow, c), dtype=torch.bfloat16, device=x.device)
+    assert out.dtype == torch.bfloat16 and out.is_contiguous() and tuple(out.shape[:3]) == (n, oh, ow) and out.shape[3] >= c_off + c
+    _call("ladi_pool2d_bf16", 0.0, _ptr(x), n, h, w, c, pitch, k, s, p, mode, _ptr(out), out.shape[3], c_off, _stream())
+    return out
+
+
+def global_avg_pool(x):
+    """adaptive_avg_pool2d(x, 1).flatten(1): NHWC bf16 -> fp32 [n, C]."""
+    n, h, w, c, pitch = _nhwc(x)
+    out = torch.empty((n, c), dtype=torch.float32, device=x.device)
+    _call("ladi_pool2d_bf16", 0.0, _ptr(x), n, h, w, c, pitch, 0, 0, 0, POOL_GLOBAL_AVG_F32, _ptr(out), c, 0, _stream())
+    return out
+
+
+def lpips_layer_(fa, fb, lin, acc):
+    """acc[b] += spatial mean of lin . (unit(fa) - unit(fb))^2 for NHWC bf16 feature pairs of equal shape and pitch."""
+    n, h, w, c, pitch = _nhwc(fa)
+    assert _nhwc(fb) == (n, h, w, c, pitch) and lin.dtype == torch.float32 and lin.numel() == c and lin.is_contiguous()
+    assert acc.dtype == torch.float32 and acc.numel() == n and acc.is_contiguous()
+    _call("ladi_lpips_layer", 0.0, _ptr(fa), _ptr(fb), n, h, w, c, pitch, _ptr(lin), _ptr(acc), _stream())
+    return acc
+
+
+def ssim(x, y):
+    """Per-image SSIM (torchmetrics, data_range 1.0, gaussian 11 / 1.5) of NCHW fp32 images -> fp32 [n]."""
+    assert x.dtype == torch.float32 and y.dtype == torch.float32 and x.is_contiguous() and y.is_contiguous() and x.shape == y.shape
+    n, c, h, w = x.shape
+    tiles = lib.load().ladi_ssim_partials(h, w) if lib.RECORD is None else 1
+    if tiles < 0:
+        raise ValueError(f"SSIM needs images of at least 11 x 11 pixels, got {h} x {w}")
+    ws = torch.empty(n * tiles, dtype=torch.float32, device=x.device)
+    out = torch.empty(n, dtype=torch.float32, device=x.device)
+    _call("ladi_ssim_f32", 0.0, _ptr(x), _ptr(y), n, c, h, w, _ptr(ws), _ptr(out), _stream())
+    return out
+
+
+def resize_tf1_u8(x, oh, ow):
+    """(x * 255).byte() + torch-fidelity's TF1 bilinear resize: NCHW fp32 in [0, 1] -> NCHW fp32 [n, c, oh, ow] in [0, 255]."""
+    assert x.dtype == torch.float32 and x.is_contiguous()
+    n, c, h, w = x.shape
+    out = torch.empty((n, c, oh, ow), dtype=torch.float32, device=x.device)
+    _call("ladi_resize_tf1_u8", 0.0, _ptr(x), n, c, h, w, oh, ow, _ptr(out), _stream())
+    return out
