@@ -1,4 +1,7 @@
-"""Every distinct kernel call of the benchmarked workloads, replayed one by one against a float64 reference with per-element error bounds.
+"""Every distinct kernel call the engine modules issue in the benchmarked workloads (UNet, VAE encode and decode, EMASC, the inversion
+adapter, and the `plan_context` GEMM), replayed one by one against a float64 reference with per-element error bounds.  The kernels the
+Python sequencing issues around them (the pipeline's glue) and the inference CLI's front end (cloth warping, the CLIP towers) are
+tests/test_gpu_glue_frontend_census.py's.
 
 The census (CPU).  Plan-only engines for the full-size UNet, VAE, EMASC and inversion adapter (random weights packed on the CPU, library
 defaults: no CTA pairs, no LayerNorm fold) are walked at the shapes of bench.py / BASELINE.json; the text-context GEMM of
