@@ -273,73 +273,98 @@ convgemm_kernel(const __grid_constant__ AMaps amaps, const __grid_constant__ CUt
         }
       }
       float rs[2] = {0.f, 0.f}, rq[2] = {0.f, 0.f};  // row statistics of the current 32-column chunk (rowstat_out)
+      // Columns in groups of 32 (JG column pairs per thread).  A group's bias and residual loads are all issued before any of its
+      // arithmetic and stores: each element's branches end a basic block, so loads left inside the element code waited out one
+      // memory latency per element pair.
+      constexpr int JG = 4;
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int c = acc0 + 8 * j + 2 * q;                  // global accumulator column of this thread's pair
-        const bool v0 = c < p.c_out, v1 = c + 1 < p.c_out;
-        float b0 = 0.f, b1 = 0.f, cs0 = 0.f, cs1 = 0.f;
-        if (bias != nullptr && !p.bias_per_row) {
-          if (v0) b0 = __ldg(bias + c);
-          if (v1) b1 = __ldg(bias + c + 1);
-        }
-        if (p.ln_stats != nullptr) {
-          if (v0) cs0 = __ldg(p.ln_colsum + c);
-          if (v1) cs1 = __ldg(p.ln_colsum + c + 1);
-        }
+      for (int j0 = 0; j0 < BN / 8; j0 += JG) {
+        float bv[JG][2];
+        uint32_t rv[JG][2];
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
-          if (p.ln_stats != nullptr) { f0 = fmaf(ln_b[h], cs0, ln_a[h] * f0); f1 = fmaf(ln_b[h], cs1, ln_a[h] * f1); }
-          if (p.bias_per_row) { f0 += rbias[h]; f1 += rbias[h]; }
-          else { f0 += b0; f1 += b1; }
-          if (p.act == 2) {  // GEGLU: interleaved (value, gate) pair -> one output column
-            if (row_ok[h] && v1)
-              reinterpret_cast<bf16*>(p.out)[orow[h] * p.out_pitch + (c >> 1)] = __float2bfloat16(f0 * gelu_erf(f1) * rscale[h]);
-            continue;
-          }
-          if (p.act == 1) { f0 = silu_f(f0); f1 = silu_f(f1); }
-          else if (p.act == 3) { f0 = gelu_erf(f0); f1 = gelu_erf(f1); }
-          else if (p.act == 4) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
-          // The residual is read through the read-only path (__ldg).  Plain loads might alias the output stores of the earlier
-          // columns, so the compiler had to keep them behind those stores in the unrolled epilogue.  With the stores and loads free
-          // to reorder, conv/GEMM time per denoising step fell from 37.9 to 32.0 ms (H100 80GB HBM3, 400 W, the bench.py workload),
-          // and launches without a residual share that code and got faster too.  An in-place residual (residual == out) stays
-          // correct: each element is read only by the thread that later writes it.
-          if (p.residual != nullptr && row_ok[h]) {
-            const bf16* rr = p.residual + grow[h] * p.residual_pitch + c;
-            if (v1 && (p.residual_pitch & 1) == 0) {
-              const uint32_t u = __ldg(reinterpret_cast<const unsigned int*>(rr));
-              f0 += ptx::bf16_lo(u); f1 += ptx::bf16_hi(u);
-            } else {
-              if (v0) f0 += __bfloat162float(__ldg(rr));
-              if (v1) f1 += __bfloat162float(__ldg(rr + 1));
-            }
-          }
-          if (p.rowstat_out != nullptr) {
-            rs[h] += f0 + f1;
-            rq[h] = fmaf(f0, f0, fmaf(f1, f1, rq[h]));
-          }
-          f0 *= rscale[h]; f1 *= rscale[h];
-          if (!row_ok[h]) continue;
-          if (p.out_fp32) {
-            float* o = reinterpret_cast<float*>(p.out) + (size_t)split * p.split_stride + orow[h] * p.out_pitch + c;
-            if (v1 && (p.out_pitch & 1) == 0) *reinterpret_cast<float2*>(o) = make_float2(f0, f1);
-            else { if (v0) o[0] = f0; if (v1) o[1] = f1; }
-          } else {
-            bf16* o = reinterpret_cast<bf16*>(p.out) + orow[h] * p.out_pitch + c;
-            if (v1 && (p.out_pitch & 1) == 0) *reinterpret_cast<uint32_t*>(o) = ptx::pack_bf16(f0, f1);
-            else { if (v0) o[0] = __float2bfloat16(f0); if (v1) o[1] = __float2bfloat16(f1); }
-          }
-        }
-        if (p.rowstat_out != nullptr && (j & 3) == 3) {     // a 32-column chunk is complete: reduce over the 4 lanes of the row
+        for (int jj = 0; jj < JG; ++jj) {
+          const int c = acc0 + 8 * (j0 + jj) + 2 * q;
+          const bool v0 = c < p.c_out, v1 = c + 1 < p.c_out;
+          bv[jj][0] = (bias != nullptr && !p.bias_per_row && v0) ? __ldg(bias + c) : 0.f;
+          bv[jj][1] = (bias != nullptr && !p.bias_per_row && v1) ? __ldg(bias + c + 1) : 0.f;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            float s_ = rs[h], q_ = rq[h];
-            s_ += __shfl_xor_sync(0xffffffffu, s_, 1); q_ += __shfl_xor_sync(0xffffffffu, q_, 1);
-            s_ += __shfl_xor_sync(0xffffffffu, s_, 2); q_ += __shfl_xor_sync(0xffffffffu, q_, 2);
-            const int chunk_col = acc0 + 8 * (j - 3);
-            if (q == 0 && row_ok[h] && chunk_col < p.c_out) p.rowstat_out[grow[h] * p.rowstat_chunks + (chunk_col >> 5)] = make_float2(s_, q_);
-            rs[h] = 0.f; rq[h] = 0.f;
+            uint32_t u = 0u;
+            if (p.residual != nullptr && row_ok[h]) {
+              const bf16* rr = p.residual + grow[h] * p.residual_pitch + c;
+              if (v1 && (p.residual_pitch & 1) == 0) {
+                u = __ldg(reinterpret_cast<const unsigned int*>(rr));
+              } else {
+                const uint32_t lo = v0 ? (uint32_t)__ldg(reinterpret_cast<const unsigned short*>(rr)) : 0u;
+                const uint32_t hi = v1 ? (uint32_t)__ldg(reinterpret_cast<const unsigned short*>(rr) + 1) : 0u;
+                u = lo | (hi << 16);
+              }
+            }
+            rv[jj][h] = u;
+          }
+        }
+#pragma unroll
+        for (int jj = 0; jj < JG; ++jj) {
+          const int j = j0 + jj;
+          const int c = acc0 + 8 * j + 2 * q;                  // global accumulator column of this thread's pair
+          const bool v0 = c < p.c_out, v1 = c + 1 < p.c_out;
+          const float b0 = bv[jj][0], b1 = bv[jj][1];
+          float cs0 = 0.f, cs1 = 0.f;
+          if (p.ln_stats != nullptr) {
+            if (v0) cs0 = __ldg(p.ln_colsum + c);
+            if (v1) cs1 = __ldg(p.ln_colsum + c + 1);
+          }
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+            if (p.ln_stats != nullptr) { f0 = fmaf(ln_b[h], cs0, ln_a[h] * f0); f1 = fmaf(ln_b[h], cs1, ln_a[h] * f1); }
+            if (p.bias_per_row) { f0 += rbias[h]; f1 += rbias[h]; }
+            else { f0 += b0; f1 += b1; }
+            if (p.act == 2) {  // GEGLU: interleaved (value, gate) pair -> one output column
+              if (row_ok[h] && v1)
+                reinterpret_cast<bf16*>(p.out)[orow[h] * p.out_pitch + (c >> 1)] = __float2bfloat16(f0 * gelu_erf(f1) * rscale[h]);
+              continue;
+            }
+            if (p.act == 1) { f0 = silu_f(f0); f1 = silu_f(f1); }
+            else if (p.act == 3) { f0 = gelu_erf(f0); f1 = gelu_erf(f1); }
+            else if (p.act == 4) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+            // The residual is read through the read-only path (__ldg), preloaded above.  An in-place residual (residual == out) stays
+            // correct: each element is read only by the thread that later writes it, and before it writes it.
+            if (p.residual != nullptr && row_ok[h]) {
+              const uint32_t u = rv[jj][h];
+              if (v1 && (p.residual_pitch & 1) == 0) {
+                f0 += ptx::bf16_lo(u); f1 += ptx::bf16_hi(u);
+              } else {
+                if (v0) f0 += ptx::bf16_lo(u);
+                if (v1) f1 += ptx::bf16_hi(u);
+              }
+            }
+            if (p.rowstat_out != nullptr) {
+              rs[h] += f0 + f1;
+              rq[h] = fmaf(f0, f0, fmaf(f1, f1, rq[h]));
+            }
+            f0 *= rscale[h]; f1 *= rscale[h];
+            if (!row_ok[h]) continue;
+            if (p.out_fp32) {
+              float* o = reinterpret_cast<float*>(p.out) + (size_t)split * p.split_stride + orow[h] * p.out_pitch + c;
+              if (v1 && (p.out_pitch & 1) == 0) *reinterpret_cast<float2*>(o) = make_float2(f0, f1);
+              else { if (v0) o[0] = f0; if (v1) o[1] = f1; }
+            } else {
+              bf16* o = reinterpret_cast<bf16*>(p.out) + orow[h] * p.out_pitch + c;
+              if (v1 && (p.out_pitch & 1) == 0) *reinterpret_cast<uint32_t*>(o) = ptx::pack_bf16(f0, f1);
+              else { if (v0) o[0] = __float2bfloat16(f0); if (v1) o[1] = __float2bfloat16(f1); }
+            }
+          }
+          if (p.rowstat_out != nullptr && (j & 3) == 3) {     // a 32-column chunk is complete: reduce over the 4 lanes of the row
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float s_ = rs[h], q_ = rq[h];
+              s_ += __shfl_xor_sync(0xffffffffu, s_, 1); q_ += __shfl_xor_sync(0xffffffffu, q_, 1);
+              s_ += __shfl_xor_sync(0xffffffffu, s_, 2); q_ += __shfl_xor_sync(0xffffffffu, q_, 2);
+              const int chunk_col = acc0 + 8 * (j - 3);
+              if (q == 0 && row_ok[h] && chunk_col < p.c_out) p.rowstat_out[grow[h] * p.rowstat_chunks + (chunk_col >> 5)] = make_float2(s_, q_);
+              rs[h] = 0.f; rq[h] = 0.f;
+            }
           }
         }
       }
