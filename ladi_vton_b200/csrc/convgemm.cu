@@ -1,7 +1,8 @@
 // Implicit-GEMM convolution / GEMM for sm_90a: TMA (4-D shifted boxes, zero OOB fill = conv padding) -> 128B-swizzled smem
 // -> wgmma (bf16 x bf16 -> fp32 in registers) -> fused epilogue (bias / per-step bias / SiLU / GEGLU / residual / row scale /
-// LayerNorm fold / row statistics) -> bf16 or fp32 NHWC, stored from the accumulator fragment.  Persistent CTAs, one per SM;
-// warpgroup 0 = TMA producer, warpgroups 1-2 = MMA + epilogue (64 rows each).
+// LayerNorm fold / row statistics) -> bf16 or fp32 NHWC.  bf16 rows of whole 16-byte chunks go through a shared-memory staging tile
+// and leave as 16-byte stores (staged_epilogue, the epilogue form fixed at compile time); everything else is stored from the
+// accumulator fragment.  Persistent CTAs, one per SM; warpgroup 0 = TMA producer, warpgroups 1-2 = MMA + epilogue (64 rows each).
 //
 // Replaces, on the reference hot path: every nn.Conv2d / nn.Linear executed by UNet2DConditionModel.forward
 // (src/vto_pipelines/tryon_pipe.py:732), AutoencoderKL.encode/decode (src/models/vae.py:99-119,183-212) and
@@ -60,6 +61,8 @@ struct KParams {
   // nearest-2x upsample fused into a 3x3 convolution (diffusers Upsample2D): the 4 output parities are 4 groups of M tiles, each a
   // 2x2-tap convolution over the half-resolution input with its own merged weights and a strided output tensor map
   int up2x, tiles_pp;         // tiles_pp = M tiles per parity plane
+  // staged epilogue (bf16 out, 16-byte rows; see staged_epilogue): 0 = fragment stores; form = act | residual << 3 | column bias << 4
+  int staged, form;
 };
 
 struct AMaps {
@@ -112,10 +115,127 @@ __device__ __forceinline__ TileCoord tile_coord(const KParams& p, int tile) {
   return t;
 }
 
+// Staged epilogue: the BM x BN bf16 tile goes through shared memory and leaves as whole 16-byte chunks per output row.
+// Staging layout: row r (of the 128 tile rows) is BN * 2 bytes; its 16-byte chunk c sits at chunk c ^ f(r), so that the 8 rows a
+// stmatrix / ldmatrix matrix addresses, and the 8 consecutive chunks a quarter-warp drains, hit 8 distinct bank groups.
+template <int BN>
+__device__ __forceinline__ uint32_t stage_off(int r, int c) {
+  const int pc = BN >= 64 ? (c ^ (r & 7)) : (c ^ ((r >> 1) & 3));  // BN = 32: 64-byte rows, two per 128-byte bank window
+  return (uint32_t)(r * (BN * 2) + pc * 16);
+}
+constexpr int STAGE_ROWTAB_BYTES = BM * 8;  // per tile row: output pixel index, or -1 past the extent
+
+// One consumer warpgroup's 64 rows, with the epilogue form fixed at compile time: per element act(acc + bias) (+ residual) * row scale,
+// one rounding to bf16, in the order and with the functions of the fragment epilogue (bit-identical results).  ACT as KParams::act;
+// COLBIAS: a per-column bias, else the per-row bias (0 without a bias).  No per-element test is left: columns at or past c_out (whole
+// 8-column groups, c_out % 8 == 0) and rows past the extent are computed on whatever the staging tile holds and are not stored.
+// rowtab holds the output pixel of every tile row (or -1); the caller wrote it and synchronised the warpgroup.
+template <int BN, int ACT, bool RES, bool COLBIAS>
+__device__ __forceinline__ void staged_epilogue(const KParams& p, const float (&acc)[BN / 2], const float* bias, int acc0, uint32_t sstage,
+                                                uint32_t rowtab, int cw, const float (&rscale)[2], const float (&rbias)[2]) {
+  constexpr int CPR = BN / 8;                         // 16-byte chunks per staged row
+  constexpr int OCPR = ACT == 2 ? CPR / 2 : CPR;      // ... per output row (GEGLU: half width)
+  const int tid = threadIdx.x & 127, warp = tid >> 5, lane = tid & 31, q = lane & 3;
+  const int r0 = 64 * cw;
+  if constexpr (RES) {
+    // the residual of this warpgroup's rows, coalesced 16-byte loads into the staging tile.  residual rows are output rows (no up2x).
+    // An in-place residual (residual == out) stays correct: these elements are written only by this warpgroup's drain below.
+    constexpr int NV = 64 * CPR / 128;
+    uint4 v[NV];
+#pragma unroll
+    for (int k = 0; k < NV; ++k) {
+      const int i = tid + 128 * k, r = r0 + i / CPR, col = acc0 + 8 * (i % CPR);
+      const long long o = ptx::ld_shared_s64(rowtab + 8 * r);
+      v[k] = (o >= 0 && col < p.c_out) ? __ldg(reinterpret_cast<const uint4*>(p.residual + (size_t)o * p.residual_pitch + col))
+                                       : make_uint4(0u, 0u, 0u, 0u);
+    }
+#pragma unroll
+    for (int k = 0; k < NV; ++k) {
+      const int i = tid + 128 * k;
+      ptx::st_shared_v4(sstage + stage_off<BN>(r0 + i / CPR, i % CPR), v[k]);
+    }
+    ptx::named_barrier_sync(1 + cw, 128);
+  }
+  // stmatrix / ldmatrix matrix m = lane / 8 of column groups (j, j+1): rows + 8 * (m & 1), group j + (m >> 1)
+  const int wrow = r0 + 16 * (warp & 3);
+  const int mrow = wrow + 8 * ((lane >> 3) & 1) + (lane & 7);
+#pragma unroll
+  for (int j = 0; j < BN / 8; j += 2) {
+    float b[2][2];
+#pragma unroll
+    for (int jj = 0; jj < 2; ++jj) {
+      const int c = acc0 + 8 * (j + jj) + 2 * q;
+      float2 bb = make_float2(0.f, 0.f);
+      if (COLBIAS && c < p.c_out) bb = __ldg(reinterpret_cast<const float2*>(bias + c));
+      b[jj][0] = bb.x; b[jj][1] = bb.y;
+    }
+    uint32_t res[4];
+    const uint32_t maddr = sstage + stage_off<BN>(mrow, j + (lane >> 4));
+    if constexpr (RES) ptx::ldmatrix_x4(maddr, res);
+    uint32_t packed[4];
+#pragma unroll
+    for (int m = 0; m < 4; ++m) {
+      const int h = m & 1, jj = m >> 1;
+      float f0 = acc[4 * (j + jj) + 2 * h], f1 = acc[4 * (j + jj) + 2 * h + 1];
+      if constexpr (COLBIAS) { f0 += b[jj][0]; f1 += b[jj][1]; }
+      else { f0 += rbias[h]; f1 += rbias[h]; }
+      if constexpr (ACT == 2) {  // GEGLU: (value, gate) pair -> output column 4 (j + jj) + q of the half-width tile
+        const bf16 g = __float2bfloat16(f0 * gelu_erf(f1) * rscale[h]);
+        ptx::st_shared_b16(sstage + stage_off<BN>(wrow + 8 * h + (lane >> 2), (j + jj) >> 1) + 2 * (4 * ((j + jj) & 1) + q),
+                           __bfloat16_as_ushort(g));
+        continue;
+      }
+      if constexpr (ACT == 1) { f0 = silu_f(f0); f1 = silu_f(f1); }
+      if constexpr (ACT == 3) { f0 = gelu_erf(f0); f1 = gelu_erf(f1); }
+      if constexpr (ACT == 4) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+      if constexpr (RES) { f0 += ptx::bf16_lo(res[m]); f1 += ptx::bf16_hi(res[m]); }
+      f0 *= rscale[h]; f1 *= rscale[h];
+      packed[m] = ptx::pack_bf16(f0, f1);
+    }
+    if constexpr (ACT != 2) ptx::stmatrix_x4(maddr, packed);
+  }
+  ptx::named_barrier_sync(1 + cw, 128);
+  // drain: this warpgroup's 64 rows, consecutive threads on consecutive 16-byte chunks of a row
+  constexpr int NO = 64 * OCPR / 128;
+  const int ocols = ACT == 2 ? p.c_out >> 1 : p.c_out, oc0 = ACT == 2 ? acc0 >> 1 : acc0;
+  uint4 v[NO];
+#pragma unroll
+  for (int k = 0; k < NO; ++k) {
+    const int i = tid + 128 * k;
+    v[k] = ptx::ld_shared_v4(sstage + stage_off<BN>(r0 + i / OCPR, i % OCPR));
+  }
+#pragma unroll
+  for (int k = 0; k < NO; ++k) {
+    const int i = tid + 128 * k, col = oc0 + 8 * (i % OCPR);
+    const long long o = ptx::ld_shared_s64(rowtab + 8 * (r0 + i / OCPR));
+    if (o >= 0 && col < ocols) *reinterpret_cast<uint4*>(reinterpret_cast<bf16*>(p.out) + (size_t)o * p.out_pitch + col) = v[k];
+  }
+}
+
+// The staged epilogue body of the launch's form (one branch per tile).
+template <int BN>
+__device__ __forceinline__ void staged_dispatch(const KParams& p, const float (&acc)[BN / 2], const float* bias, int acc0, uint32_t sstage,
+                                                uint32_t rowtab, int cw, const float (&rscale)[2], const float (&rbias)[2]) {
+#define LADI_STAGED_FORM(A, R, B) \
+  case (A) | ((R) << 3) | ((B) << 4): staged_epilogue<BN, A, R, B>(p, acc, bias, acc0, sstage, rowtab, cw, rscale, rbias); break;
+#define LADI_STAGED_ACT(A) LADI_STAGED_FORM(A, 0, 0) LADI_STAGED_FORM(A, 0, 1) LADI_STAGED_FORM(A, 1, 0) LADI_STAGED_FORM(A, 1, 1)
+  switch (p.form) {
+    LADI_STAGED_ACT(0)
+    LADI_STAGED_ACT(1)
+    LADI_STAGED_FORM(2, 0, 0)
+    LADI_STAGED_FORM(2, 0, 1)
+    LADI_STAGED_ACT(3)
+    LADI_STAGED_ACT(4)
+    default: __trap();
+  }
+#undef LADI_STAGED_ACT
+#undef LADI_STAGED_FORM
+}
+
 // One CTA = one 128-row M tile x BN columns at a time, persistent over work items.  Warpgroup 0: TMA producer (one warp issues);
 // warpgroups 1 and 2: wgmma consumers, each owning 64 of the 128 rows with its fp32 accumulator in registers, followed by the
-// fused epilogue straight from the accumulator fragment.  The producer runs ahead into the next work item's K blocks while the
-// consumers are in their epilogue.
+// fused epilogue (staged, or straight from the accumulator fragment).  The producer runs ahead into the next work item's K blocks
+// while the consumers are in their epilogue.
 // PAIR = true: clusters of two CTAs on two M tiles of the same N tile.  Each CTA loads its own A tile and HALF of the B rows,
 // multicast into the shared memory of both CTAs, so every B tile crosses L2 -> SM once per pair instead of once per CTA.  A stage
 // is refilled only after the consumers of BOTH CTAs have released it.
@@ -126,7 +246,10 @@ convgemm_kernel(const __grid_constant__ AMaps amaps, const __grid_constant__ CUt
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int B_BYTES = BN * BK * 2;
   const int STAGES = p.stages;
-  uint8_t* sA = smem;
+  constexpr int STAGE_BYTES = BM * BN * 2;
+  // [staging tile][row table] only for a staged launch, then the pipeline stages and their barriers
+  const uint32_t sstage = ptx::smem_u32(smem), rowtab = sstage + STAGE_BYTES;
+  uint8_t* sA = smem + (p.staged ? STAGE_BYTES + STAGE_ROWTAB_BYTES : 0);
   uint8_t* sB = sA + STAGES * A_BYTES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sB + STAGES * B_BYTES);
   const uint32_t full0 = ptx::smem_u32(bars), empty0 = full0 + 8 * MAX_STAGES;
@@ -270,6 +393,18 @@ convgemm_kernel(const __grid_constant__ AMaps amaps, const __grid_constant__ CUt
           const float var = fmaxf(q_ * inv_c - mean * mean, 0.f);
           ln_a[h] = rsqrtf(var + p.ln_eps);
           ln_b[h] = -ln_a[h] * mean;
+        }
+      }
+      if constexpr (!PAIR && BN <= 128) {
+        if (p.staged) {
+          ptx::named_barrier_sync(1 + cw, 128);  // the previous tile's drain has read the staging tile and the row table
+          if (q == 0) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) ptx::st_shared_s64(rowtab + 8 * (rbase + 8 * h), row_ok[h] ? (long long)orow[h] : -1ll);
+          }
+          ptx::named_barrier_sync(1 + cw, 128);
+          staged_dispatch<BN>(p, acc, bias, acc0, sstage, rowtab, cw, rscale, rbias);
+          continue;
         }
       }
       float rs[2] = {0.f, 0.f}, rq[2] = {0.f, 0.f};  // row statistics of the current 32-column chunk (rowstat_out)
@@ -431,11 +566,12 @@ int launch(const AMaps& am, const CUtensorMap& tmB, KParams& kp, cudaStream_t st
     attr_set = true;
   }
   const size_t per_stage = A_BYTES + (size_t)BN * BK * 2;
-  int stages = (int)((SMEM_LIMIT - SMEM_TAIL) / per_stage);
+  const size_t staging = kp.staged ? (size_t)BM * BN * 2 + STAGE_ROWTAB_BYTES : 0;
+  int stages = (int)((SMEM_LIMIT - SMEM_TAIL - staging) / per_stage);
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   LADI_CHECK(stages >= 2, "not enough shared memory for a 2-stage pipeline");
   kp.stages = stages;
-  const size_t smem = stages * per_stage + SMEM_TAIL;
+  const size_t smem = staging + stages * per_stage + SMEM_TAIL;
   if (PAIR) {
     const int items = ((kp.tiles_m + 1) / 2) * kp.tiles_n;
     const int clusters = items < max_clusters ? items : max_clusters;
@@ -629,6 +765,18 @@ extern "C" int ladi_conv2d_bf16(const ladi_conv_desc* d, void* stream_) {
     else if (d->pair_mode == 0 && ladi_conv_pair_default()) pair = kp.tiles_m >= 4 && (kp.tiles_m % 2 == 0 || kp.tiles_m >= 16);
   }
   LADI_CHECK(d->pair_mode != 1 || pair, "pair_mode=1 needs >= 2 M tiles, BN >= 128 and no split-K (BN=%d, tiles_m=%d)", BN, kp.tiles_m);
+
+  // ---- epilogue: staged through shared memory (16-byte stores) for bf16 rows of whole, aligned 16-byte chunks; fragment stores for
+  // fp32 / split-K partials, the LayerNorm fold and row statistics, odd widths, CTA pairs and N tiles wider than 128
+  {
+    const int out_cols = d->act == 2 ? d->c_out / 2 : d->c_out;
+    const bool col_bias = d->bias != nullptr && !d->bias_per_row;
+    kp.staged = !pair && !split && BN <= 128 && !d->out_fp32 && d->rowstat_out == nullptr && d->ln_stats == nullptr &&
+                out_cols % 8 == 0 && d->c_out % 8 == 0 && d->out_pitch % 8 == 0 && reinterpret_cast<uintptr_t>(d->out) % 16 == 0 &&
+                (d->residual == nullptr || (d->residual_pitch % 8 == 0 && reinterpret_cast<uintptr_t>(d->residual) % 16 == 0)) &&
+                (!col_bias || (reinterpret_cast<uintptr_t>(d->bias) % 8 == 0 && d->bias_step_stride % 2 == 0));
+    kp.form = d->act | (d->residual != nullptr ? 1 << 3 : 0) | (col_bias ? 1 << 4 : 0);
+  }
 
   CUtensorMap tmB;
   {

@@ -117,6 +117,41 @@ __device__ __forceinline__ void named_barrier_arrive(uint32_t id, uint32_t nthre
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// ----------------------------------------------------------------------------------------------- shared-memory loads / stores
+__device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint4 v) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+__device__ __forceinline__ void st_shared_b16(uint32_t addr, uint16_t v) {
+  asm volatile("st.shared.b16 [%0], %1;" ::"r"(addr), "h"(v) : "memory");
+}
+__device__ __forceinline__ long long ld_shared_s64(uint32_t addr) {
+  long long v;
+  asm volatile("ld.shared.s64 %0, [%1];" : "=l"(v) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_shared_s64(uint32_t addr, long long v) {
+  asm volatile("st.shared.s64 [%0], %1;" ::"r"(addr), "l"(v) : "memory");
+}
+
+// ----------------------------------------------------------------------------------------------- ldmatrix / stmatrix
+// Four 8x8 b16 matrices; lanes 8m..8m+7 address the 8 rows (16 bytes each) of matrix m.  Register m of lane t holds row t/4,
+// columns 2(t%4) and 2(t%4)+1 of matrix m: the wgmma accumulator fragment layout of an 8-column group.
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+
 // ----------------------------------------------------------------------------------------------- wgmma (warpgroup MMA)
 // Shared-memory matrix descriptor (sm_90), 128-byte swizzle: start[0,14) LBO[16,30) SBO[32,46) base_offset[49,52)=0
 // layout_type[62,64)=1 (SWIZZLE_128B); addresses and offsets in units of 16 bytes.  Tiles are 1024-byte aligned.
