@@ -83,8 +83,10 @@ typedef struct ladi_conv_desc {
   void* out;
   int out_pitch;
   int out_fp32;
-  int force_bn;              /* 0 = auto; else N tile in {32,64,128,160,192,256} (tests / tuning) */
-  int force_direct_epilogue; /* accepted for ABI compatibility; sm_90a has one epilogue (stores from the accumulator fragment) */
+  int force_bn;              /* 0 = the library chooses the N tile (and may split K); else this N tile, one of {32,64,128,160,192,256},
+                                without split-K (tests / tuning) */
+  int force_direct_epilogue; /* accepted and ignored (kept for ABI compatibility): the store path, staged through shared memory or from
+                                the accumulator fragment, is chosen from the rest of the descriptor */
   void* splitk_ws;           /* optional fp32 workspace: enables split-K for few-tile / long-K shapes (NULL = never split) */
   int64_t splitk_ws_bytes;
   int pair_mode;             /* CTA pairs (2-CTA clusters on two M tiles of one N tile; each CTA loads half of the B tile and multicasts

@@ -96,6 +96,33 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return 0.5f * x * (1.f + copysignf(e, x));
 }
 
+// The per-element epilogue, defined here once for the three places that apply it (staged_epilogue, the fragment epilogue of
+// convgemm_kernel, splitk_reduce_kernel), which only supply the operands and store the result.  In this order, in fp32:
+//   v = acc (after the LayerNorm fold) + bias;  v = act(v);  v += residual;  [row statistics are taken of v here]  v *= row scale;
+// then ONE rounding to bf16.  GEGLU instead maps an interleaved (value, gate) column pair to one output and takes no residual.
+// ACT as KParams::act: 0 none, 1 SiLU, 3 GELU(erf), 4 ReLU (2 = GEGLU is geglu_f).
+template <int ACT>
+__device__ __forceinline__ float act_f(float x) {
+  if constexpr (ACT == 1) return silu_f(x);
+  else if constexpr (ACT == 3) return gelu_erf(x);
+  else if constexpr (ACT == 4) return fmaxf(x, 0.f);
+  else return x;
+}
+__device__ __forceinline__ float geglu_f(float value, float gate, float rscale) { return value * gelu_erf(gate) * rscale; }
+// act_f of a runtime `act` on every element given: one test per call, not per element.  `act` by reference, so that each test reads
+// the kernel parameter where the caller holds it (passing a copy moved the basic blocks of two instantiations around).
+template <typename... F>
+__device__ __forceinline__ void act_rt(const int& act, F&... v) {
+  if (act == 1) ((v = act_f<1>(v)), ...);
+  else if (act == 3) ((v = act_f<3>(v)), ...);
+  else if (act == 4) ((v = act_f<4>(v)), ...);
+}
+// the bias row of the current denoising step: bias table [steps][bias_step_stride], *step_ptr advanced on the device
+__device__ __forceinline__ const float* step_bias(const float* bias, const int* step_ptr, int bias_step_stride) {
+  if (bias != nullptr && step_ptr != nullptr) bias += (size_t)(*step_ptr) * bias_step_stride;
+  return bias;
+}
+
 struct TileCoord {
   int nt, x0, y0, n0, par;
 };
@@ -115,6 +142,40 @@ __device__ __forceinline__ TileCoord tile_coord(const KParams& p, int tile) {
   return t;
 }
 
+// Row r (0..127) of a tile = pixel (n, y, x) of the bn x bh x bw box.  ok: inside the output extent; grow: its index in the tile grid's
+// plane (the row of residual, row_scale, per-row bias and both statistics tables); orow: in the output tensor (differs only with up2x).
+struct TileRow { bool ok; size_t grow, orow; };
+__device__ __forceinline__ TileRow tile_row(const KParams& p, const TileCoord& tc, int r) {
+  const int rn = r / (p.bh * p.bw), rr = r - rn * (p.bh * p.bw);
+  const int ry = rr / p.bw, rx = rr - ry * p.bw;
+  const int n = tc.n0 + rn, y = tc.y0 + ry, x = tc.x0 + rx;
+  TileRow t;
+  t.ok = (n < p.n_img) && (y < p.H) && (x < p.W);
+  t.grow = ((size_t)n * p.H + y) * p.W + x;
+  // up2x: plane pixel (y, x) of output parity par is pixel (2y + py, 2x + px) of the full-resolution output
+  t.orow = p.up2x ? ((size_t)n * 2 * p.H + 2 * y + (tc.par >> 1)) * (2 * p.W) + 2 * x + (tc.par & 1) : t.grow;
+  return t;
+}
+
+// Folded LayerNorm, consumer side: {rstd, -rstd * mean} of A row `row` from the producer's per-chunk partial sums, summed in chunk
+// order (deterministic).  {1, 0} without ln_stats.
+__device__ __forceinline__ float2 ln_fold_row(const KParams& p, const TileRow& row) {
+  if (p.ln_stats == nullptr) return make_float2(1.f, 0.f);
+  float s_ = 0.f, q_ = 0.f;
+  if (row.ok) {
+    const float4* st = reinterpret_cast<const float4*>(p.ln_stats + row.grow * p.ln_chunks);  // ln_chunks is even
+    for (int c = 0; c < (p.ln_chunks >> 1); ++c) {
+      const float4 u = __ldg(st + c);
+      s_ += u.x; q_ += u.y; s_ += u.z; q_ += u.w;
+    }
+  }
+  const float inv_c = 1.f / (32.f * (float)p.ln_chunks);
+  const float mean = s_ * inv_c;
+  const float var = fmaxf(q_ * inv_c - mean * mean, 0.f);
+  const float rstd = rsqrtf(var + p.ln_eps);
+  return make_float2(rstd, -rstd * mean);
+}
+
 // Staged epilogue: the BM x BN bf16 tile goes through shared memory and leaves as whole 16-byte chunks per output row.
 // Staging layout: row r (of the 128 tile rows) is BN * 2 bytes; its 16-byte chunk c sits at chunk c ^ f(r), so that the 8 rows a
 // stmatrix / ldmatrix matrix addresses, and the 8 consecutive chunks a quarter-warp drains, hit 8 distinct bank groups.
@@ -125,8 +186,7 @@ __device__ __forceinline__ uint32_t stage_off(int r, int c) {
 }
 constexpr int STAGE_ROWTAB_BYTES = BM * 8;  // per tile row: output pixel index, or -1 past the extent
 
-// One consumer warpgroup's 64 rows, with the epilogue form fixed at compile time: per element act(acc + bias) (+ residual) * row scale,
-// one rounding to bf16, in the order and with the functions of the fragment epilogue (bit-identical results).  ACT as KParams::act;
+// One consumer warpgroup's 64 rows, with the epilogue form fixed at compile time (per element as stated at act_f).  ACT as KParams::act;
 // COLBIAS: a per-column bias, else the per-row bias (0 without a bias).  No per-element test is left: columns at or past c_out (whole
 // 8-column groups, c_out % 8 == 0) and rows past the extent are computed on whatever the staging tile holds and are not stored.
 // rowtab holds the output pixel of every tile row (or -1); the caller wrote it and synchronised the warpgroup.
@@ -180,14 +240,12 @@ __device__ __forceinline__ void staged_epilogue(const KParams& p, const float (&
       if constexpr (COLBIAS) { f0 += b[jj][0]; f1 += b[jj][1]; }
       else { f0 += rbias[h]; f1 += rbias[h]; }
       if constexpr (ACT == 2) {  // GEGLU: (value, gate) pair -> output column 4 (j + jj) + q of the half-width tile
-        const bf16 g = __float2bfloat16(f0 * gelu_erf(f1) * rscale[h]);
+        const bf16 g = __float2bfloat16(geglu_f(f0, f1, rscale[h]));
         ptx::st_shared_b16(sstage + stage_off<BN>(wrow + 8 * h + (lane >> 2), (j + jj) >> 1) + 2 * (4 * ((j + jj) & 1) + q),
                            __bfloat16_as_ushort(g));
         continue;
       }
-      if constexpr (ACT == 1) { f0 = silu_f(f0); f1 = silu_f(f1); }
-      if constexpr (ACT == 3) { f0 = gelu_erf(f0); f1 = gelu_erf(f1); }
-      if constexpr (ACT == 4) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+      f0 = act_f<ACT>(f0); f1 = act_f<ACT>(f1);
       if constexpr (RES) { f0 += ptx::bf16_lo(res[m]); f1 += ptx::bf16_hi(res[m]); }
       f0 *= rscale[h]; f1 *= rscale[h];
       packed[m] = ptx::pack_bf16(f0, f1);
@@ -329,8 +387,7 @@ convgemm_kernel(const __grid_constant__ AMaps amaps, const __grid_constant__ CUt
         if constexpr (PAIR) ptx::mbar_arrive_cluster(empty_peer0 + 8 * st);
       }
     };
-    const float* bias = p.bias;
-    if (bias != nullptr && p.step_ptr != nullptr) bias += (size_t)(*p.step_ptr) * p.bias_step_stride;
+    const float* bias = step_bias(p.bias, p.step_ptr, p.bias_step_stride);
     const int q = lane & 3;
     const int rbase = 64 * cw + 16 * (warp & 3) + (lane >> 2);  // this thread's rows: rbase and rbase + 8
     uint32_t stage = 0, phase = 0;
@@ -358,55 +415,34 @@ convgemm_kernel(const __grid_constant__ AMaps amaps, const __grid_constant__ CUt
       ptx::reg_fence(acc);
       release(prev);
 
-      // ---------------------------------------------------------------- epilogue from the accumulator fragment
+      // ---------------------------------------------------------------- epilogue, both store paths: this thread's two rows of the tile
       const TileCoord tc = tile_coord(p, tile);
       const int acc0 = tc.nt * BN;                           // first accumulator column of this tile (global)
-      bool row_ok[2];
-      size_t grow[2], orow[2];
-      float rscale[2], rbias[2], ln_a[2], ln_b[2];
+      TileRow row[2];
+      float rscale[2], rbias[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int r = rbase + 8 * h;
-        const int rn = r / (p.bh * p.bw), rr = r - rn * (p.bh * p.bw);
-        const int ry = rr / p.bw, rx = rr - ry * p.bw;
-        const int n = tc.n0 + rn, y = tc.y0 + ry, x = tc.x0 + rx;
-        row_ok[h] = (n < p.n_img) && (y < p.H) && (x < p.W);
-        grow[h] = ((size_t)n * p.H + y) * p.W + x;
-        // up2x: plane pixel (y, x) of output parity par is pixel (2y + py, 2x + px) of the full-resolution output
-        orow[h] = p.up2x ? ((size_t)n * 2 * p.H + 2 * y + (tc.par >> 1)) * (2 * p.W) + 2 * x + (tc.par & 1) : grow[h];
-        rscale[h] = (p.row_scale != nullptr && row_ok[h]) ? p.row_scale[grow[h]] : 1.f;
-        rbias[h] = (p.bias_per_row && bias != nullptr && row_ok[h]) ? bias[grow[h]] : 0.f;
-        // folded LayerNorm (consumer side): mean / rstd of this A row from the producer's per-chunk partial sums, summed in chunk
-        // order (deterministic)
-        ln_a[h] = 1.f; ln_b[h] = 0.f;
-        if (p.ln_stats != nullptr) {
-          float s_ = 0.f, q_ = 0.f;
-          if (row_ok[h]) {
-            const float4* st = reinterpret_cast<const float4*>(p.ln_stats + grow[h] * p.ln_chunks);  // ln_chunks is even
-            for (int c = 0; c < (p.ln_chunks >> 1); ++c) {
-              const float4 u = __ldg(st + c);
-              s_ += u.x; q_ += u.y; s_ += u.z; q_ += u.w;
-            }
-          }
-          const float inv_c = 1.f / (32.f * (float)p.ln_chunks);
-          const float mean = s_ * inv_c;
-          const float var = fmaxf(q_ * inv_c - mean * mean, 0.f);
-          ln_a[h] = rsqrtf(var + p.ln_eps);
-          ln_b[h] = -ln_a[h] * mean;
-        }
+        row[h] = tile_row(p, tc, rbase + 8 * h);
+        rscale[h] = (p.row_scale != nullptr && row[h].ok) ? p.row_scale[row[h].grow] : 1.f;
+        rbias[h] = (p.bias_per_row && bias != nullptr && row[h].ok) ? bias[row[h].grow] : 0.f;
       }
+      // ---------------------------------------------------------------- staged: row table, then the body of the launch's form
       if constexpr (!PAIR && BN <= 128) {
         if (p.staged) {
           ptx::named_barrier_sync(1 + cw, 128);  // the previous tile's drain has read the staging tile and the row table
           if (q == 0) {
 #pragma unroll
-            for (int h = 0; h < 2; ++h) ptx::st_shared_s64(rowtab + 8 * (rbase + 8 * h), row_ok[h] ? (long long)orow[h] : -1ll);
+            for (int h = 0; h < 2; ++h) ptx::st_shared_s64(rowtab + 8 * (rbase + 8 * h), row[h].ok ? (long long)row[h].orow : -1ll);
           }
           ptx::named_barrier_sync(1 + cw, 128);
           staged_dispatch<BN>(p, acc, bias, acc0, sstage, rowtab, cw, rscale, rbias);
           continue;
         }
       }
+      // ---------------------------------------------------------------- fragment: stores from the accumulator, forms tested per element
+      float2 ln[2];                                  // out = ln.x * acc + ln.y * colsum[c] (+ bias)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) ln[h] = ln_fold_row(p, row[h]);
       float rs[2] = {0.f, 0.f}, rq[2] = {0.f, 0.f};  // row statistics of the current 32-column chunk (rowstat_out)
       // Columns in groups of 32 (JG column pairs per thread).  A group's bias and residual loads are all issued before any of its
       // arithmetic and stores: each element's branches end a basic block, so loads left inside the element code waited out one
@@ -425,8 +461,8 @@ convgemm_kernel(const __grid_constant__ AMaps amaps, const __grid_constant__ CUt
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             uint32_t u = 0u;
-            if (p.residual != nullptr && row_ok[h]) {
-              const bf16* rr = p.residual + grow[h] * p.residual_pitch + c;
+            if (p.residual != nullptr && row[h].ok) {
+              const bf16* rr = p.residual + row[h].grow * p.residual_pitch + c;
               if (v1 && (p.residual_pitch & 1) == 0) {
                 u = __ldg(reinterpret_cast<const unsigned int*>(rr));
               } else {
@@ -452,20 +488,18 @@ convgemm_kernel(const __grid_constant__ AMaps amaps, const __grid_constant__ CUt
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
-            if (p.ln_stats != nullptr) { f0 = fmaf(ln_b[h], cs0, ln_a[h] * f0); f1 = fmaf(ln_b[h], cs1, ln_a[h] * f1); }
+            if (p.ln_stats != nullptr) { f0 = fmaf(ln[h].y, cs0, ln[h].x * f0); f1 = fmaf(ln[h].y, cs1, ln[h].x * f1); }
             if (p.bias_per_row) { f0 += rbias[h]; f1 += rbias[h]; }
             else { f0 += b0; f1 += b1; }
             if (p.act == 2) {  // GEGLU: interleaved (value, gate) pair -> one output column
-              if (row_ok[h] && v1)
-                reinterpret_cast<bf16*>(p.out)[orow[h] * p.out_pitch + (c >> 1)] = __float2bfloat16(f0 * gelu_erf(f1) * rscale[h]);
+              if (row[h].ok && v1)
+                reinterpret_cast<bf16*>(p.out)[row[h].orow * p.out_pitch + (c >> 1)] = __float2bfloat16(geglu_f(f0, f1, rscale[h]));
               continue;
             }
-            if (p.act == 1) { f0 = silu_f(f0); f1 = silu_f(f1); }
-            else if (p.act == 3) { f0 = gelu_erf(f0); f1 = gelu_erf(f1); }
-            else if (p.act == 4) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+            act_rt(p.act, f0, f1);
             // The residual is read through the read-only path (__ldg), preloaded above.  An in-place residual (residual == out) stays
             // correct: each element is read only by the thread that later writes it, and before it writes it.
-            if (p.residual != nullptr && row_ok[h]) {
+            if (p.residual != nullptr && row[h].ok) {
               const uint32_t u = rv[jj][h];
               if (v1 && (p.residual_pitch & 1) == 0) {
                 f0 += ptx::bf16_lo(u); f1 += ptx::bf16_hi(u);
@@ -479,13 +513,13 @@ convgemm_kernel(const __grid_constant__ AMaps amaps, const __grid_constant__ CUt
               rq[h] = fmaf(f0, f0, fmaf(f1, f1, rq[h]));
             }
             f0 *= rscale[h]; f1 *= rscale[h];
-            if (!row_ok[h]) continue;
+            if (!row[h].ok) continue;
             if (p.out_fp32) {
-              float* o = reinterpret_cast<float*>(p.out) + (size_t)split * p.split_stride + orow[h] * p.out_pitch + c;
+              float* o = reinterpret_cast<float*>(p.out) + (size_t)split * p.split_stride + row[h].orow * p.out_pitch + c;
               if (v1 && (p.out_pitch & 1) == 0) *reinterpret_cast<float2*>(o) = make_float2(f0, f1);
               else { if (v0) o[0] = f0; if (v1) o[1] = f1; }
             } else {
-              bf16* o = reinterpret_cast<bf16*>(p.out) + orow[h] * p.out_pitch + c;
+              bf16* o = reinterpret_cast<bf16*>(p.out) + row[h].orow * p.out_pitch + c;
               if (v1 && (p.out_pitch & 1) == 0) *reinterpret_cast<uint32_t*>(o) = ptx::pack_bf16(f0, f1);
               else { if (v0) o[0] = __float2bfloat16(f0); if (v1) o[1] = __float2bfloat16(f1); }
             }
@@ -497,7 +531,7 @@ convgemm_kernel(const __grid_constant__ AMaps amaps, const __grid_constant__ CUt
               s_ += __shfl_xor_sync(0xffffffffu, s_, 1); q_ += __shfl_xor_sync(0xffffffffu, q_, 1);
               s_ += __shfl_xor_sync(0xffffffffu, s_, 2); q_ += __shfl_xor_sync(0xffffffffu, q_, 2);
               const int chunk_col = acc0 + 8 * (j - 3);
-              if (q == 0 && row_ok[h] && chunk_col < p.c_out) p.rowstat_out[grow[h] * p.rowstat_chunks + (chunk_col >> 5)] = make_float2(s_, q_);
+              if (q == 0 && row[h].ok && chunk_col < p.c_out) p.rowstat_out[row[h].grow * p.rowstat_chunks + (chunk_col >> 5)] = make_float2(s_, q_);
               rs[h] = 0.f; rq[h] = 0.f;
             }
           }
@@ -516,7 +550,7 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restr
                                                             const int* __restrict__ step_ptr, int act, const bf16* __restrict__ residual,
                                                             int residual_pitch, bf16* __restrict__ out, int out_pitch) {
   ptx::pdl_wait();
-  if (bias != nullptr && step_ptr != nullptr) bias += (size_t)(*step_ptr) * bias_step_stride;
+  bias = step_bias(bias, step_ptr, bias_step_stride);
   const int cv = c_out >> 2;
   const long long total = rows * cv;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -531,9 +565,7 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restr
       const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + col));
       acc.x += b4.x; acc.y += b4.y; acc.z += b4.z; acc.w += b4.w;
     }
-    if (act == 1) { acc.x = silu_f(acc.x); acc.y = silu_f(acc.y); acc.z = silu_f(acc.z); acc.w = silu_f(acc.w); }
-    if (act == 3) { acc.x = gelu_erf(acc.x); acc.y = gelu_erf(acc.y); acc.z = gelu_erf(acc.z); acc.w = gelu_erf(acc.w); }
-    if (act == 4) { acc.x = fmaxf(acc.x, 0.f); acc.y = fmaxf(acc.y, 0.f); acc.z = fmaxf(acc.z, 0.f); acc.w = fmaxf(acc.w, 0.f); }
+    act_rt(act, acc.x, acc.y, acc.z, acc.w);
     if (residual != nullptr) {
       const uint2 u = __ldg(reinterpret_cast<const uint2*>(residual + row * residual_pitch + col));
       acc.x += ptx::bf16_lo(u.x); acc.y += ptx::bf16_hi(u.x); acc.z += ptx::bf16_lo(u.y); acc.w += ptx::bf16_hi(u.y);
@@ -590,16 +622,7 @@ int largest_pow2_divisor(int v, int cap) {
   return d;
 }
 
-int encode_nhwc_map(CUtensorMap* m, const void* base, int channels, int pitch, int w, int h, int n, const uint32_t* box, int swz) {
-  const uint64_t dims[4] = {(uint64_t)channels, (uint64_t)w, (uint64_t)h, (uint64_t)n};
-  const uint64_t strides[3] = {(uint64_t)pitch * 2, (uint64_t)pitch * 2 * w, (uint64_t)pitch * 2 * w * h};
-  return ladi_encode_tmap_bf16(m, base, 4, dims, strides, box, swz);
-}
-
-}  // namespace
-
-extern "C" int ladi_conv2d_bf16(const ladi_conv_desc* d, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+int validate(const ladi_conv_desc* d) {
   LADI_CHECK(d != nullptr, "conv desc is null");
   LADI_CHECK(d->ksize == 1 || d->ksize == 3, "ksize must be 1 or 3 (got %d)", d->ksize);
   LADI_CHECK(d->stride == 1 || d->stride == 2, "stride must be 1 or 2 (got %d)", d->stride);
@@ -608,7 +631,7 @@ extern "C" int ladi_conv2d_bf16(const ladi_conv_desc* d, void* stream_) {
   LADI_CHECK(d->act >= 0 && d->act <= 4, "bad act");
   LADI_CHECK(d->act != 2 || (d->c_out % 2 == 0 && !d->out_fp32 && d->residual == nullptr), "GEGLU needs even c_out, bf16 out");
   LADI_CHECK(d->out != nullptr && d->weight != nullptr, "null out/weight");
-  const int up = d->up2x ? 1 : 0;
+  const bool up = d->up2x != 0;
   if (up) {
     LADI_CHECK(d->ksize == 3 && d->stride == 1 && d->n_sc == 0, "up2x: 3x3 stride-1 convolution without fused shortcut only");
     LADI_CHECK(d->h_out % 2 == 0 && d->w_out % 2 == 0, "up2x: output extent must be even");
@@ -620,11 +643,13 @@ extern "C" int ladi_conv2d_bf16(const ladi_conv_desc* d, void* stream_) {
   LADI_CHECK(d->ln_stats == nullptr || (d->ln_colsum != nullptr && d->c_out % 32 == 0 && d->ksize == 1 && d->n_src == 1 && d->n_sc == 0 &&
                                         d->src_c[0] % 64 == 0 && !d->out_fp32 && !d->bias_per_row && !up),
              "ln_stats: GEMM over one source of K %% 64 == 0, c_out %% 32 == 0, bf16 out, ln_colsum given");
+  return LADI_OK;
+}
 
-  KParams kp;
-  memset(&kp, 0, sizeof(kp));
-  AMaps am;
-  // up2x: the tile grid covers ONE output parity plane (h_out/2 x w_out/2 pixels = the input extent); tiles_m counts all four
+// The M tile (bn x bh x bw pixels) and the tile grid.  up2x: the grid covers ONE output parity plane (h_out/2 x w_out/2 pixels = the
+// input extent); tiles_m counts all four.
+void tile_geometry(const ladi_conv_desc* d, KParams& kp) {
+  const int up = d->up2x ? 1 : 0;
   const int HO = up ? d->h_out / 2 : d->h_out, WO = up ? d->w_out / 2 : d->w_out;
   kp.n_img = d->n; kp.H = HO; kp.W = WO; kp.c_out = d->c_out;
   kp.bw = largest_pow2_divisor(WO, 128);
@@ -637,41 +662,52 @@ extern "C" int ladi_conv2d_bf16(const ladi_conv_desc* d, void* stream_) {
   kp.tiles_m = kp.tiles_x * kp.tiles_y * kp.tiles_b;
   kp.up2x = up; kp.tiles_pp = kp.tiles_m;
   if (up) kp.tiles_m *= 4;
+}
 
-  // ---- A tensor maps: one per (source, parity plane)
-  int nmaps = 0;
-  const int s = d->stride;
-  const int h_in = up ? HO : (d->h_in > 0 ? d->h_in : d->h_out * s), w_in = up ? WO : (d->w_in > 0 ? d->w_in : d->w_out * s);
+// A tensor maps, one per (source, parity plane) and per shortcut source, and the K segments that walk them: taps (row-major) x
+// sources, then the shortcut sources.  Weight K order must match (see packer).
+int build_a_maps_and_segments(const ladi_conv_desc* d, KParams& kp, AMaps& am) {
+  const int up = kp.up2x, s = d->stride;
+  const int h_in = up ? kp.H : (d->h_in > 0 ? d->h_in : d->h_out * s), w_in = up ? kp.W : (d->w_in > 0 ? d->w_in : d->w_out * s);
   const uint32_t box[4] = {(uint32_t)BK, (uint32_t)kp.bw, (uint32_t)kp.bh, (uint32_t)kp.bn};
-  int src_map0[2] = {0, 0}, sc_map0[2] = {0, 0};
+  int nmaps = 0, src_map0[2] = {0, 0}, sc_map0[2] = {0, 0};
+  // the st x st parity planes of one NHWC tensor (st = 1: the tensor itself)
+  auto add_maps = [&](const void* ptr, int c, int pitch_, int w, int h, int st) -> int {
+    for (int py = 0; py < st; ++py)
+      for (int px = 0; px < st; ++px) {
+        LADI_CHECK(nmaps < NUM_A_MAPS, "too many tensor maps");
+        const uint64_t pitch = (uint64_t)pitch_;
+        const uint64_t dims[4] = {(uint64_t)c, (uint64_t)((w - px + st - 1) / st), (uint64_t)((h - py + st - 1) / st), (uint64_t)d->n};
+        const uint64_t strides[3] = {pitch * 2 * st, pitch * 2 * w * st, pitch * 2 * (uint64_t)w * h};
+        const bf16* base = reinterpret_cast<const bf16*>(ptr) + ((size_t)py * w + px) * pitch;
+        if (ladi_encode_tmap_bf16(&am.m[nmaps++], base, 4, dims, strides, box)) return LADI_ERR_CUDA;
+      }
+    return LADI_OK;
+  };
   for (int i = 0; i < d->n_src; ++i) {
     LADI_CHECK(d->src[i] != nullptr && d->src_c[i] > 0 && d->src_pitch[i] % 8 == 0 && d->src_pitch[i] >= d->src_c[i],
                "source %d: need non-null, pitch multiple of 8 and >= C", i);
     src_map0[i] = nmaps;
-    for (int py = 0; py < s; ++py)
-      for (int px = 0; px < s; ++px) {
-        LADI_CHECK(nmaps < NUM_A_MAPS, "too many tensor maps");
-        const uint64_t pitch = (uint64_t)d->src_pitch[i];
-        const uint64_t dims[4] = {(uint64_t)d->src_c[i], (uint64_t)((w_in - px + s - 1) / s), (uint64_t)((h_in - py + s - 1) / s),
-                                  (uint64_t)d->n};
-        const uint64_t strides[3] = {pitch * 2 * s, pitch * 2 * w_in * s, pitch * 2 * (uint64_t)w_in * h_in};
-        const bf16* base = reinterpret_cast<const bf16*>(d->src[i]) + ((size_t)py * w_in + px) * pitch;
-        if (ladi_encode_tmap_bf16(&am.m[nmaps], base, 4, dims, strides, box)) return LADI_ERR_CUDA;
-        ++nmaps;
-      }
+    if (const int rc = add_maps(d->src[i], d->src_c[i], d->src_pitch[i], w_in, h_in, s)) return rc;
   }
   for (int i = 0; i < d->n_sc; ++i) {
     LADI_CHECK(s == 1, "fused 1x1 shortcut requires stride 1");
     LADI_CHECK(d->sc[i] != nullptr && d->sc_c[i] > 0 && d->sc_pitch[i] % 8 == 0, "shortcut source %d invalid", i);
-    LADI_CHECK(nmaps < NUM_A_MAPS, "too many tensor maps");
     sc_map0[i] = nmaps;
-    if (encode_nhwc_map(&am.m[nmaps], d->sc[i], d->sc_c[i], d->sc_pitch[i], d->w_out, d->h_out, d->n, box, 128)) return LADI_ERR_CUDA;
-    ++nmaps;
+    if (const int rc = add_maps(d->sc[i], d->sc_c[i], d->sc_pitch[i], d->w_out, d->h_out, 1)) return rc;
   }
   for (int i = nmaps; i < NUM_A_MAPS; ++i) am.m[i] = am.m[0];
 
-  // ---- K segments: taps (row-major) x sources, then the shortcut sources.  Weight K order must match (see packer).
   int nseg = 0, total = 0;
+  auto add_seg = [&](int map, int dx, int dy, int channels) -> int {
+    LADI_CHECK(nseg < MAX_SEG, "too many K segments");
+    Segment& sg = kp.seg[nseg++];
+    sg.map = (int16_t)map; sg.dx = (int16_t)dx; sg.dy = (int16_t)dy;
+    sg.chunks = (int16_t)((channels + BK - 1) / BK);
+    sg.c_begin = 0;
+    total += sg.chunks;
+    return LADI_OK;
+  };
   const int taps = up ? 4 : d->ksize * d->ksize;
   for (int t = 0; t < taps; ++t) {
     const int ky = up ? t / 2 : (d->ksize == 3 ? t / 3 : 0), kx = up ? t % 2 : (d->ksize == 3 ? t % 3 : 0);
@@ -679,128 +715,139 @@ extern "C" int ladi_conv2d_bf16(const ladi_conv_desc* d, void* stream_) {
     // up2x: output pixel 2i+p reads input pixels i+p-1 and i+p (merged taps); the kernel adds the parity p, so the base shift is t-1
     const int oy = up ? ky - 1 : ky - (d->ksize == 3 ? d->pad_lo : 0), ox = up ? kx - 1 : kx - (d->ksize == 3 ? d->pad_lo : 0);
     const int py = ((oy % s) + s) % s, px = ((ox % s) + s) % s;
-    const int dy = (oy - py) / s, dx = (ox - px) / s;
-    for (int i = 0; i < d->n_src; ++i) {
-      LADI_CHECK(nseg < MAX_SEG, "too many K segments");
-      Segment& sg = kp.seg[nseg++];
-      sg.map = (int16_t)(src_map0[i] + py * s + px);
-      sg.dx = (int16_t)dx; sg.dy = (int16_t)dy;
-      sg.chunks = (int16_t)((d->src_c[i] + BK - 1) / BK);
-      sg.c_begin = 0;
-      total += sg.chunks;
-    }
+    for (int i = 0; i < d->n_src; ++i)
+      if (const int rc = add_seg(src_map0[i] + py * s + px, (ox - px) / s, (oy - py) / s, d->src_c[i])) return rc;
   }
-  for (int i = 0; i < d->n_sc; ++i) {
-    LADI_CHECK(nseg < MAX_SEG, "too many K segments");
-    Segment& sg = kp.seg[nseg++];
-    sg.map = (int16_t)sc_map0[i]; sg.dx = 0; sg.dy = 0;
-    sg.chunks = (int16_t)((d->sc_c[i] + BK - 1) / BK);
-    sg.c_begin = 0;
-    total += sg.chunks;
-  }
+  for (int i = 0; i < d->n_sc; ++i)
+    if (const int rc = add_seg(sc_map0[i], 0, 0, d->sc_c[i])) return rc;
   kp.nseg = nseg; kp.total_kb = total;
   LADI_CHECK(d->k_total == total * BK, "weight K (%d) != %d K-blocks x 64 implied by the sources", d->k_total, total);
   LADI_CHECK(d->weight_pitch % 8 == 0 && d->weight_pitch >= d->k_total, "weight pitch must be a multiple of 8 and >= K");
+  return LADI_OK;
+}
 
+// The path one descriptor takes: the ONLY place that decides it.  Reads nothing but its arguments.
+struct Plan {
+  int bn, splits, kb_per_split;  // N tile; split-K (splits > 1: fp32 partials, splitk_reduce_kernel runs the epilogue), as in KParams
+  bool pair, staged;             // CTA pairs; staged epilogue (else fragment stores)
+  int form;                      // KParams::form
+};
+Plan choose_plan(const ladi_conv_desc* d, int tiles_m, int total_kb, int sms) {
+  const bool up = d->up2x != 0;
+  Plan pl = {0, 1, total_kb, false, false, 0};
+  // ---- N tile.  1. the caller's (force_bn, which also rules out split-K)
+  if (d->force_bn > 0) pl.bn = d->force_bn;
+  // 2. split-K: few output tiles but a long reduction (the 8x6 / 16x12 UNet levels): spread K over otherwise idle SMs, fp32 partial
+  // planes in the caller's workspace, summed (in split order) by splitk_reduce_kernel.  Its N tile is the widest that c_out fills.
+  if (d->splitk_ws != nullptr && d->force_bn == 0 && !d->out_fp32 && d->act != 2 && d->row_scale == nullptr && !d->bias_per_row && !up &&
+      d->rowstat_out == nullptr && d->ln_stats == nullptr &&
+      d->c_out % 4 == 0 && d->out_pitch % 4 == 0 && (d->residual == nullptr || d->residual_pitch % 4 == 0) && total_kb >= 32) {
+    const int bn_s = d->c_out >= 256 ? 256 : (d->c_out >= 128 ? 128 : 64);
+    const long tiles_s = (long)tiles_m * ((d->c_out + bn_s - 1) / bn_s);
+    if (tiles_s * 2 <= sms) {
+      int S = (int)(sms / tiles_s);
+      if (S > total_kb / 8) S = total_kb / 8;
+      if (S > 16) S = 16;
+      if (S >= 2) {
+        const int per = (total_kb + S - 1) / S;
+        S = (total_kb + per - 1) / per;
+        if (S >= 2 && (long long)S * d->n * d->h_out * d->w_out * d->c_out * 4 <= d->splitk_ws_bytes) {
+          pl.bn = bn_s; pl.splits = S; pl.kb_per_split = per;
+        }
+      }
+    }
+  }
+  // 3. else minimise (waves x per-tile cost) with per-tile cost ~ BN + fixed A-operand cost.  Tiles wider than 128 (160-256, still
+  // available through force_bn) made the default workload slower on H100 (2850 vs 2450 ms per call, 512x384, batch 8, CFG, 400 W card;
+  // 160 alone as an automatic candidate: 2602 vs 2455 ms).
+  if (pl.bn == 0) {
+    static const int cand[3] = {128, 64, 32};
+    long best = -1;
+    for (int i = 0; i < 3; ++i) {
+      if (d->pair_mode == 1 && cand[i] < 128) continue;  // forced CTA pairs need a tile they can split
+      if (total_kb <= 8 && d->c_out >= 128 && cand[i] < 128) continue;  // short reductions (K <= 512): the full-width tile
+      const long tiles = (long)tiles_m * ((d->c_out + cand[i] - 1) / cand[i]);
+      const long cost = ((tiles + sms - 1) / sms) * (cand[i] + 64);
+      if (best < 0 || cost < best) { best = cost; pl.bn = cand[i]; }
+    }
+  }
+  const bool split = pl.splits > 1;
+  // ---- CTA pairs (2-CTA clusters sharing the B tile by TMA multicast): two M tiles per cluster share one N tile; needs >= 2 M tiles,
+  // no split-K, and a B half of whole 8-row swizzle groups.  pair_mode: 0 = library default (off: measured slower than single CTAs on
+  // H100 for the UNet's shapes; env LADI_CONV_2CTA=1 turns it on), 1 = force, 2 = never.  up2x: a pair shares one parity's weights, so
+  // the M tiles of a parity plane (tiles_m / 4) must pair up.
+  if (!split && tiles_m >= 2 && pl.bn >= 128 && pl.bn % 16 == 0 && (!up || (tiles_m / 4) % 2 == 0)) {
+    if (d->pair_mode == 1) pl.pair = true;
+    // default: pair whenever there are enough M tiles that the phantom tile of an odd count is noise
+    else if (d->pair_mode == 0 && ladi_conv_pair_default()) pl.pair = tiles_m >= 4 && (tiles_m % 2 == 0 || tiles_m >= 16);
+  }
+  // ---- epilogue: staged through shared memory (16-byte stores) for bf16 rows of whole, aligned 16-byte chunks; fragment stores for
+  // fp32 / split-K partials, the LayerNorm fold and row statistics, odd widths, CTA pairs and N tiles wider than 128
+  const int out_cols = d->act == 2 ? d->c_out / 2 : d->c_out;
+  const bool col_bias = d->bias != nullptr && !d->bias_per_row;
+  pl.staged = !pl.pair && !split && pl.bn <= 128 && !d->out_fp32 && d->rowstat_out == nullptr && d->ln_stats == nullptr &&
+              out_cols % 8 == 0 && d->c_out % 8 == 0 && d->out_pitch % 8 == 0 && reinterpret_cast<uintptr_t>(d->out) % 16 == 0 &&
+              (d->residual == nullptr || (d->residual_pitch % 8 == 0 && reinterpret_cast<uintptr_t>(d->residual) % 16 == 0)) &&
+              (!col_bias || (reinterpret_cast<uintptr_t>(d->bias) % 8 == 0 && d->bias_step_stride % 2 == 0));
+  pl.form = d->act | (d->residual != nullptr ? 1 << 3 : 0) | (col_bias ? 1 << 4 : 0);
+  return pl;
+}
+
+int encode_b_map(const ladi_conv_desc* d, const Plan& pl, CUtensorMap* tmB) {
+  const uint64_t dims[2] = {(uint64_t)d->k_total, (uint64_t)d->c_out * (d->up2x ? 4 : 1)};  // up2x: the four parities' merged weights, stacked
+  const uint64_t strides[1] = {(uint64_t)d->weight_pitch * 2};
+  const uint32_t bbox[2] = {(uint32_t)BK, (uint32_t)(pl.pair ? pl.bn / 2 : pl.bn)};
+  return ladi_encode_tmap_bf16(tmB, d->weight, 2, dims, strides, bbox) ? LADI_ERR_CUDA : LADI_OK;
+}
+
+// The kernel of the plan's (BN, pair), then the split-K second pass with the descriptor's own epilogue operands.
+int launch_plan(const ladi_conv_desc* d, const Plan& pl, const AMaps& am, const CUtensorMap& tmB, KParams& kp, cudaStream_t stream) {
+  using Launch = int (*)(const AMaps&, const CUtensorMap&, KParams&, cudaStream_t);
+  static const struct { int bn; Launch single, pair; } table[6] = {  // every instantiation there is; tiles below 128 do not pair
+      {256, launch<256, false>, launch<256, true>}, {192, launch<192, false>, launch<192, true>},
+      {160, launch<160, false>, launch<160, true>}, {128, launch<128, false>, launch<128, true>},
+      {64, launch<64, false>, nullptr},             {32, launch<32, false>, nullptr}};
+  Launch fn = nullptr;
+  for (const auto& e : table)
+    if (e.bn == pl.bn) fn = pl.pair ? e.pair : e.single;
+  LADI_CHECK(fn != nullptr, "unsupported BN %d", pl.bn);
+  const int rc = fn(am, tmB, kp, stream);
+  if (rc != LADI_OK || pl.splits == 1) return rc;
+  const long long rows = (long long)d->n * d->h_out * d->w_out, vecs = rows * (d->c_out / 4);
+  long long blocks = (vecs + 255) / 256;
+  if (blocks > (long long)ladi_num_sms() * 8) blocks = (long long)ladi_num_sms() * 8;
+  LADI_CUDA(ladi_launch(splitk_reduce_kernel, dim3((unsigned)blocks), dim3(256), 0, stream, (const float*)d->splitk_ws, kp.splits,
+                        kp.split_stride, rows, d->c_out, d->bias, d->bias_step_stride, d->step_ptr, d->act,
+                        reinterpret_cast<const bf16*>(d->residual), d->residual_pitch, reinterpret_cast<bf16*>(d->out), d->out_pitch));
+  return LADI_OK;
+}
+
+}  // namespace
+
+extern "C" int ladi_conv2d_bf16(const ladi_conv_desc* d, void* stream_) {
+  if (const int rc = validate(d)) return rc;
+  KParams kp;
+  memset(&kp, 0, sizeof(kp));
+  AMaps am;
+  tile_geometry(d, kp);
+  if (const int rc = build_a_maps_and_segments(d, kp, am)) return rc;
+  const Plan pl = choose_plan(d, kp.tiles_m, kp.total_kb, ladi_num_sms());
+  LADI_CHECK(d->pair_mode != 1 || pl.pair, "pair_mode=1 needs >= 2 M tiles, BN >= 128 and no split-K (BN=%d, tiles_m=%d)", pl.bn, kp.tiles_m);
+
+  // ---- the plan and the descriptor's epilogue operands -> kernel parameters
+  kp.tiles_n = (d->c_out + pl.bn - 1) / pl.bn;
+  kp.splits = pl.splits; kp.kb_per_split = pl.kb_per_split; kp.staged = pl.staged; kp.form = pl.form;
   kp.bias = d->bias; kp.bias_per_row = d->bias_per_row; kp.bias_step_stride = d->bias_step_stride; kp.step_ptr = d->step_ptr;
   kp.residual = reinterpret_cast<const bf16*>(d->residual); kp.residual_pitch = d->residual_pitch;
   kp.row_scale = d->row_scale; kp.act = d->act; kp.out = d->out; kp.out_pitch = d->out_pitch; kp.out_fp32 = d->out_fp32;
   kp.rowstat_out = reinterpret_cast<float2*>(d->rowstat_out); kp.rowstat_chunks = d->c_out / 32;
   kp.ln_stats = reinterpret_cast<const float2*>(d->ln_stats); kp.ln_chunks = d->src_c[0] / 32; kp.ln_colsum = d->ln_colsum; kp.ln_eps = d->ln_eps;
-
-  // ---- N tile: minimise (waves x per-tile cost) with per-tile cost ~ BN + fixed A-operand cost.  Tiles wider than 128 (160-256, still
-  // available through force_bn) made the default workload slower on H100 (2850 vs 2450 ms per call, 512x384, batch 8, CFG, 400 W card;
-  // 160 alone as an automatic candidate: 2602 vs 2455 ms).
-  const int sms = ladi_num_sms();
-  int BN = 0;
-  if (d->force_bn > 0) {
-    BN = d->force_bn;
-  } else {
-    static const int cand[3] = {128, 64, 32};
-    long best = -1;
-    for (int i = 0; i < 3; ++i) {
-      if (d->pair_mode == 1 && cand[i] < 128) continue;  // forced CTA pairs need a tile they can split
-      if (total <= 8 && d->c_out >= 128 && cand[i] < 128) continue;  // short reductions (K <= 512): the full-width tile
-      const long tiles = (long)kp.tiles_m * ((d->c_out + cand[i] - 1) / cand[i]);
-      const long cost = ((tiles + sms - 1) / sms) * (cand[i] + 64);
-      if (best < 0 || cost < best) { best = cost; BN = cand[i]; }
-    }
+  if (pl.splits > 1) {  // fp32 partial planes to the workspace; bias, activation and residual move to splitk_reduce_kernel
+    kp.split_stride = (long long)d->n * d->h_out * d->w_out * d->c_out;
+    kp.out = d->splitk_ws; kp.out_pitch = d->c_out; kp.out_fp32 = 1;
+    kp.bias = nullptr; kp.step_ptr = nullptr; kp.act = 0; kp.residual = nullptr;
   }
-
-  // ---- split-K: few output tiles but a long reduction (the 8x6 / 16x12 UNet levels): spread K over otherwise idle SMs,
-  // fp32 partial planes in the caller's workspace, summed (in split order) by splitk_reduce_kernel
-  kp.splits = 1; kp.kb_per_split = total; kp.split_stride = 0;
-  const long long rows = (long long)d->n * d->h_out * d->w_out;
-  bool split = false;
-  if (d->splitk_ws != nullptr && d->force_bn == 0 && !d->out_fp32 && d->act != 2 && d->row_scale == nullptr && !d->bias_per_row && !up &&
-      d->rowstat_out == nullptr && d->ln_stats == nullptr &&
-      d->c_out % 4 == 0 && d->out_pitch % 4 == 0 && (d->residual == nullptr || d->residual_pitch % 4 == 0) && total >= 32) {
-    const int bn_s = d->c_out >= 256 ? 256 : (d->c_out >= 128 ? 128 : 64);
-    const long tiles_s = (long)kp.tiles_m * ((d->c_out + bn_s - 1) / bn_s);
-    if (tiles_s * 2 <= sms) {
-      int S = (int)(sms / tiles_s);
-      if (S > total / 8) S = total / 8;
-      if (S > 16) S = 16;
-      if (S >= 2) {
-        const int per = (total + S - 1) / S;
-        S = (total + per - 1) / per;
-        if (S >= 2 && (long long)S * rows * d->c_out * 4 <= d->splitk_ws_bytes) {
-          split = true; BN = bn_s;
-          kp.splits = S; kp.kb_per_split = per; kp.split_stride = rows * d->c_out;
-          kp.out = d->splitk_ws; kp.out_pitch = d->c_out; kp.out_fp32 = 1;
-          kp.bias = nullptr; kp.step_ptr = nullptr; kp.act = 0; kp.residual = nullptr;
-        }
-      }
-    }
-  }
-  kp.tiles_n = (d->c_out + BN - 1) / BN;
-
-  // ---- CTA pairs (2-CTA clusters sharing the B tile by TMA multicast): two M tiles per cluster share one N tile; needs >= 2 M tiles,
-  // no split-K, and a B half of whole 8-row swizzle groups.  pair_mode: 0 = library default (off: measured slower than single CTAs on
-  // H100 for the UNet's shapes; env LADI_CONV_2CTA=1 turns it on), 1 = force, 2 = never.
-  bool pair = false;
-  if (!split && kp.tiles_m >= 2 && BN >= 128 && BN % 16 == 0 && (!up || kp.tiles_pp % 2 == 0)) {  // up2x: a pair shares one parity's weights
-    if (d->pair_mode == 1) pair = true;
-    // default: pair whenever there are enough M tiles that the phantom tile of an odd count is noise
-    else if (d->pair_mode == 0 && ladi_conv_pair_default()) pair = kp.tiles_m >= 4 && (kp.tiles_m % 2 == 0 || kp.tiles_m >= 16);
-  }
-  LADI_CHECK(d->pair_mode != 1 || pair, "pair_mode=1 needs >= 2 M tiles, BN >= 128 and no split-K (BN=%d, tiles_m=%d)", BN, kp.tiles_m);
-
-  // ---- epilogue: staged through shared memory (16-byte stores) for bf16 rows of whole, aligned 16-byte chunks; fragment stores for
-  // fp32 / split-K partials, the LayerNorm fold and row statistics, odd widths, CTA pairs and N tiles wider than 128
-  {
-    const int out_cols = d->act == 2 ? d->c_out / 2 : d->c_out;
-    const bool col_bias = d->bias != nullptr && !d->bias_per_row;
-    kp.staged = !pair && !split && BN <= 128 && !d->out_fp32 && d->rowstat_out == nullptr && d->ln_stats == nullptr &&
-                out_cols % 8 == 0 && d->c_out % 8 == 0 && d->out_pitch % 8 == 0 && reinterpret_cast<uintptr_t>(d->out) % 16 == 0 &&
-                (d->residual == nullptr || (d->residual_pitch % 8 == 0 && reinterpret_cast<uintptr_t>(d->residual) % 16 == 0)) &&
-                (!col_bias || (reinterpret_cast<uintptr_t>(d->bias) % 8 == 0 && d->bias_step_stride % 2 == 0));
-    kp.form = d->act | (d->residual != nullptr ? 1 << 3 : 0) | (col_bias ? 1 << 4 : 0);
-  }
-
   CUtensorMap tmB;
-  {
-    const uint64_t dims[2] = {(uint64_t)d->k_total, (uint64_t)d->c_out * (up ? 4 : 1)};  // up2x: the four parities' merged weights, stacked
-    const uint64_t strides[1] = {(uint64_t)d->weight_pitch * 2};
-    const uint32_t bbox[2] = {(uint32_t)BK, (uint32_t)(pair ? BN / 2 : BN)};
-    if (ladi_encode_tmap_bf16(&tmB, d->weight, 2, dims, strides, bbox)) return LADI_ERR_CUDA;
-  }
-  int rc = LADI_OK;
-  switch (BN) {
-    case 256: rc = pair ? launch<256, true>(am, tmB, kp, stream) : launch<256, false>(am, tmB, kp, stream); break;
-    case 192: rc = pair ? launch<192, true>(am, tmB, kp, stream) : launch<192, false>(am, tmB, kp, stream); break;
-    case 160: rc = pair ? launch<160, true>(am, tmB, kp, stream) : launch<160, false>(am, tmB, kp, stream); break;
-    case 128: rc = pair ? launch<128, true>(am, tmB, kp, stream) : launch<128, false>(am, tmB, kp, stream); break;
-    case 64: rc = launch<64, false>(am, tmB, kp, stream); break;
-    case 32: rc = launch<32, false>(am, tmB, kp, stream); break;
-    default: LADI_CHECK(false, "unsupported BN %d", BN);
-  }
-  if (rc != LADI_OK || !split) return rc;
-  const long long vecs = rows * (d->c_out / 4);
-  long long blocks = (vecs + 255) / 256;
-  if (blocks > (long long)sms * 8) blocks = (long long)sms * 8;
-  LADI_CUDA(ladi_launch(splitk_reduce_kernel, dim3((unsigned)blocks), dim3(256), 0, stream, (const float*)d->splitk_ws, kp.splits,
-                        kp.split_stride, rows, d->c_out, d->bias, d->bias_step_stride, d->step_ptr, d->act,
-                        reinterpret_cast<const bf16*>(d->residual), d->residual_pitch, reinterpret_cast<bf16*>(d->out), d->out_pitch));
-  return LADI_OK;
+  if (const int rc = encode_b_map(d, pl, &tmB)) return rc;
+  return launch_plan(d, pl, am, tmB, kp, reinterpret_cast<cudaStream_t>(stream_));
 }

@@ -41,7 +41,7 @@ def _nhwc(t):
     assert t.dim() == 4 and t.stride(3) == 1, "expect NHWC with contiguous channels"
     n, h, w, c = t.shape
     pitch = t.stride(2)
-    assert (w == 1 or True) and t.stride(1) == pitch * w and (n == 1 or t.stride(0) == pitch * w * h), \
+    assert t.stride(1) == pitch * w and (n == 1 or t.stride(0) == pitch * w * h), \
         f"non-dense NHWC view: shape {tuple(t.shape)} strides {t.stride()}"
     assert pitch % 8 == 0 and t.data_ptr() % 16 == 0, "pitch must be a multiple of 8 elements and the base 16-byte aligned"
     return n, h, w, c, pitch

@@ -25,8 +25,8 @@ def rnd(shape, dev, seed, scale=1.0):
                                       (256, 256, 384, 192), (256, 256, 512, 256), (3072, 320, 960, 0), (77 * 2, 1024, 640, 0)])
 @pytest.mark.parametrize("direct", [False, True])
 def test_gemm_plain(cuda, M, K, N, bn, direct):
-    """direct=True: sm_90a has one epilogue (stores from the accumulator fragment), so force_direct_epilogue is accepted and must leave
-    the output bit-identical."""
+    """direct=True: force_direct_epilogue is accepted and ignored (the library picks the store path, staged or fragment, from the rest of
+    the descriptor), so it must leave the output bit-identical."""
     from ladi_vton_b200 import ops, weights
     a = rnd((M, K), cuda, 1).bfloat16()
     w = rnd((N, K), cuda, 2, K ** -0.5)
