@@ -1,0 +1,105 @@
+"""The head-width-64 attention kernel at the edges of its schedule: the QK^T pipeline's prologue and drain (1, 2, 3, 4 and 24 key tiles),
+ragged last key tiles, query tails that leave some consumer warpgroups of the last query tile with few or no rows, and the fused-QKV
+projection read in place.  Each case is checked the way tests/test_gpu_workload_census.py checks the workload's calls: against float64
+with the same per-element bound, bit for bit against a second run, and with every byte of the output buffer outside the rows and columns
+the call owns (pitch gaps, the gap between batch images) NaN-poisoned before the call and still NaN after it."""
+import ctypes as C
+
+import pytest
+import torch
+
+from test_gpu_workload_census import Replay, _attn_ref, _bitwise_equal, attn_expect, ratio
+
+SCALE = 0.125
+PAD = 24  # columns of NaN after each row of every operand (keeps the pitch a multiple of 8)
+GAP = 40  # NaN elements between consecutive batch images
+
+
+def _operand(R, B, n, width, pitch, bstride, std, col0=0, buf=None):
+    """values [B, n, width] written at column col0 of a [B] x [n rows of `pitch`] buffer with batch stride `bstride` (NaN elsewhere)."""
+    if buf is None:
+        buf = torch.full(((B - 1) * bstride + n * pitch,), float("nan"), dtype=torch.bfloat16, device=R.dev)
+    vals = (R.randn(B, n, width) * std).bfloat16()
+    buf.as_strided((B, n, width), (bstride, pitch, 1), col0).copy_(vals)
+    return buf, vals
+
+
+def run_case(R, B, heads, nq, nkv, fused=False):
+    from ladi_vton_b200 import lib
+    width = heads * 64
+    d = lib.AttnDesc()
+    d.batch, d.heads, d.nq, d.nkv, d.scale, d.variant = B, heads, nq, nkv, SCALE, 0
+    if fused:  # one [B][n][3 * width + PAD] projection output: q, k, v are column slices of it
+        assert nq == nkv
+        pitch = 3 * width + PAD
+        bs = nq * pitch + GAP
+        buf, q = _operand(R, B, nq, width, pitch, bs, 2 ** 0.5)
+        _, k = _operand(R, B, nq, width, pitch, bs, 2 ** 0.5, col0=width, buf=buf)
+        _, v = _operand(R, B, nq, width, pitch, bs, 1.0, col0=2 * width, buf=buf)
+        base = buf.data_ptr()
+        d.q, d.k, d.v = base, base + 2 * width, base + 4 * width
+        d.q_pitch = d.k_pitch = d.v_pitch = pitch
+        d.q_batch_stride = d.k_batch_stride = d.v_batch_stride = bs
+        keep = [buf]
+    else:
+        pitch = width + PAD
+        qb, q = _operand(R, B, nq, width, pitch, nq * pitch + GAP, 2 ** 0.5)
+        kb, k = _operand(R, B, nkv, width, pitch, nkv * pitch + GAP, 2 ** 0.5)
+        vb, v = _operand(R, B, nkv, width, pitch, nkv * pitch + GAP, 1.0)
+        d.q, d.q_pitch, d.q_batch_stride = qb.data_ptr(), pitch, nq * pitch + GAP
+        d.k, d.k_pitch, d.k_batch_stride = kb.data_ptr(), pitch, nkv * pitch + GAP
+        d.v, d.v_pitch, d.v_batch_stride = vb.data_ptr(), pitch, nkv * pitch + GAP
+        keep = [qb, kb, vb]
+    op, obs = width + PAD, nq * (width + PAD) + GAP
+    d.out_pitch, d.out_batch_stride = op, obs
+    outs = []
+    for _ in range(2):
+        o = torch.full(((B - 1) * obs + nq * op,), float("nan"), dtype=torch.bfloat16, device=R.dev)
+        d.out = o.data_ptr()
+        lib.call("ladi_attention_bf16", C.byref(d), R.stream)
+        outs.append(o)
+    torch.cuda.synchronize()
+    del keep
+    out = outs[0]
+    owned = torch.zeros(out.shape, dtype=torch.bool, device=R.dev)
+    owned.as_strided((B, nq, width), (obs, op, 1)).fill_(True)
+    assert bool(torch.isfinite(out[owned].float()).all()), "unwritten or NaN-contaminated output element"
+    assert bool(torch.isnan(out[~owned].float()).all()), "wrote outside its rows and columns (pitch gap or batch gap)"
+    assert _bitwise_equal(outs[0], outs[1]), "two runs differ bitwise"
+    ov = out.as_strided((B, nq, width), (obs, op, 1))
+    for b in range(B):
+        o64, sv = _attn_ref(q[b].double(), k[b].double(), v[b].double(), heads, 64, SCALE)
+        worst = float(ratio(ov[b], o64, attn_expect(o64, sv, nkv)).max())
+        assert worst <= 1.0, f"image {b}: err/bound {worst:.3g}"
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("n_tiles", [1, 2, 3, 4, 24])
+def test_key_tile_counts(cuda, n_tiles):
+    run_case(Replay(cuda, 10 + n_tiles), 2, 2, 200, 128 * n_tiles)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("nkv", [77, 129, 255])
+def test_ragged_last_key_tile(cuda, nkv):
+    run_case(Replay(cuda, 40 + nkv), 2, 3, 192, nkv)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("nq", [1, 48, 64, 65, 128, 200, 260, 383])
+def test_query_tails(cuda, nq):
+    run_case(Replay(cuda, 70 + nq), 3, 2, nq, 300)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("n", [96, 333])
+def test_fused_qkv_in_place(cuda, n):
+    run_case(Replay(cuda, 90 + n), 2, 5, n, n, fused=True)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("B, heads, nq, nkv", [(8, 8, 400, 300), (16, 10, 200, 77), (6, 5, 1000, 129)])
+def test_persistent_ctas_run_several_items(cuda, B, heads, nq, nkv):
+    # more (query tile, head, image) items than an H100 has SMs: CTAs carry the K / V ring, the Q double buffer and the warpgroups'
+    # issue order from one item into the next
+    run_case(Replay(cuda, B * heads + nq + nkv), B, heads, nq, nkv)

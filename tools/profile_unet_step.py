@@ -4,7 +4,7 @@
 Builds the pipeline the way bench.py does (512x384, batch 8, CFG: UNet batch 16), runs one call, then traces ONE replay of the captured
 step graph with torch.profiler (CUDA activities).  The kernels are joined, in launch order, with the engine's plan-mode op trace
 (ladi_engine_trace) of the same UNet forward: every convgemm_kernel launch is one `conv` record (a split-K reduce belongs to the
-conv before it).  Kernel times are exclusive, as in bench.py's in_graph figures: with programmatic dependent launch a kernel starts
+conv before it), and every attention kernel launch is one `attn` record.  Kernel times are exclusive, as in bench.py's in_graph figures: with programmatic dependent launch a kernel starts
 while its predecessor drains, and only the part after the predecessor's end is charged to it.
 
 Writes OUT/profile.json (one row per launch) and OUT/profile.txt (launches and descriptors sorted by time), with the card's name and
@@ -39,6 +39,14 @@ def parse_conv(line):
     form = "+".join(x for x in [ACT[i("act")], "res" if i("res") else "", "rowscale" if i("rs") else "",
                                 "rowbias" if i("bpr") else "", "stepbias" if i("bss") else "", "fp32" if i("f32") else ""] if x) or "bias"
     return dict(kind=kind, level=f"{i('h')}x{i('w')}", M=M, N=N, K=k_true, form=form, flop=2.0 * M * N * k_true, hbm_bytes=hbm)
+
+
+def parse_attn(line):
+    f = {k: int(v) for k, v in re.findall(r"(\w+)=(\d+)\b(?![.@])", line) if k in ("d", "batch", "heads", "nq", "nkv")}
+    B, h, nq, nkv, d = f["batch"], f["heads"], f["nq"], f["nkv"], f["d"]
+    # Q, K, V read once and O written once (bf16): the least traffic the call needs
+    return dict(kind="attn", shape=f"d={d} B={B} h={h} nq={nq} nkv={nkv}", flop=4.0 * B * h * nq * nkv * d,
+                hbm_bytes=2 * B * h * d * (2 * nq + 2 * nkv))
 
 
 def main():
@@ -82,9 +90,10 @@ def main():
     Bp = 2 * B if args.guidance > 1.0 else B
     trace = pipe.unet.engine.trace(eng.MODULE_UNET, Bp, H // 8, W // 8).splitlines()
     convs = [parse_conv(l) for l in trace if l.startswith("conv ")]
-    n_attn_trace = sum(1 for l in trace if l.startswith("attn "))
+    attns = [parse_attn(l) for l in trace if l.startswith("attn ")]
+    n_attn_trace = len(attns)
 
-    rows, prev_end, ci = [], None, 0
+    rows, prev_end, ci, ai = [], None, 0, 0
     for e in ev:
         st = e.time_range.start if prev_end is None else max(e.time_range.start, prev_end)
         us = max(0.0, e.time_range.end - st)
@@ -98,6 +107,9 @@ def main():
                      pair=m.group(2) == "true", us=us, idx=ci)
             rows.append(r)
             ci += 1
+        elif "attention_" in e.name and ai < len(attns):
+            rows.append(dict(attns[ai], module="attention", kernel=re.sub(r"\(.*", "", e.name)[-80:], us=us, idx=ai))
+            ai += 1
         elif "splitk_reduce" in e.name and rows and rows[-1].get("kernel") == "convgemm_kernel":
             rows[-1]["us"] += us
             rows[-1]["splitk_reduce"] = True
@@ -128,7 +140,7 @@ def main():
     # descriptors: identical (kind, level, M, N, K, form, BN) launches summed
     desc = {}
     for r in rows:
-        if "flop" not in r:
+        if "BN" not in r:
             continue
         key = (r["module"], r["M"], r["N"], r["K"], r["form"], r["BN"])
         d = desc.setdefault(key, dict(module=r["module"], M=r["M"], N=r["N"], K=r["K"], form=r["form"], BN=r["BN"], launches=0, us=0.0, flop=0.0))
@@ -137,16 +149,26 @@ def main():
     for d in descs:
         d["tflops"] = d["flop"] / (d["us"] * 1e-6) / 1e12 if d["us"] else None
         d["share"] = d["us"] / wall if wall else None
+    adesc = {}
+    for r in rows:
+        if "shape" in r:
+            d = adesc.setdefault(r["shape"], dict(shape=r["shape"], launches=0, us=0.0, flop=0.0))
+            d["launches"] += 1; d["us"] += r["us"]; d["flop"] += r["flop"]
+    adescs = sorted(adesc.values(), key=lambda d: -d["us"])
+    for d in adescs:
+        d["tflops"] = d["flop"] / (d["us"] * 1e-6) / 1e12 if d["us"] else None
+        d["share"] = d["us"] / wall if wall else None
     fam = {}
     for r in rows:
-        k = "conv" if "flop" in r else r["module"]
+        k = "conv" if "BN" in r else r["module"]
         fam[k] = fam.get(k, 0.0) + r["us"]
 
     os.makedirs(args.out, exist_ok=True)
     gpu = gpu_identity(0)
     res = {"gpu": gpu, "workload": f"{H}x{W}, batch {B}, UNet batch {Bp}, one replay of the step graph", "step_wall_us": wall,
            "rows_sum_us": total, "family_us": fam, "conv_launches": n_conv_k, "conv_records": len(convs), "errors": errors,
-           "peak_source": "H100 SXM data sheet: 989 TFLOP/s dense bf16, 3.35 TB/s HBM3 (700 W)", "descriptors": descs, "launches": rows}
+           "peak_source": "H100 SXM data sheet: 989 TFLOP/s dense bf16, 3.35 TB/s HBM3 (700 W)", "descriptors": descs,
+           "attention_descriptors": adescs, "launches": rows}
     with open(os.path.join(args.out, "profile.json"), "w") as f:
         json.dump(res, f, indent=1)
     lines = [f"# {gpu['name']}, power limit {gpu['power_limit']}; {res['workload']}",
@@ -156,12 +178,18 @@ def main():
     for d in descs:
         lines.append(f"{d['module']:<16}{d['M']:>7}{d['N']:>6}{d['K']:>6} {d['form']:<16}{d['BN']:>4}{d['launches']:>4}{d['us'] / 1e3:>8.3f}"
                      f"{d['tflops']:>9.1f}{100 * d['share']:>6.1f}%")
+    lines += ["", "## attention descriptors, by total time", f"{'shape':<42}{'n':>4}{'ms':>8}{'TFLOP/s':>9}{'share':>7}"]
+    for d in adescs:
+        lines.append(f"{d['shape']:<42}{d['launches']:>4}{d['us'] / 1e3:>8.3f}{d['tflops']:>9.1f}{100 * d['share']:>6.1f}%")
     lines += ["", "## launches, by time",
               f"{'#':>4} {'module':<16}{'M':>7}{'N':>6}{'K':>6} {'form':<16}{'BN':>4}{'us':>9}{'TFLOP/s':>9}{'MB':>8} {'bound':<7}{'share':>7}"]
     for r in sorted(rows, key=lambda r: -r["us"]):
-        if "flop" in r:
+        if "BN" in r:
             lines.append(f"{r['idx']:>4} {r['module']:<16}{r['M']:>7}{r['N']:>6}{r['K']:>6} {r['form']:<16}{r['BN']:>4}{r['us']:>9.1f}"
                          f"{r['tflops']:>9.1f}{r['hbm_bytes'] / 1e6:>8.1f} {r['bound']:<7}{100 * r['share']:>6.2f}%")
+        elif "shape" in r:
+            lines.append(f"{r['idx']:>4} {'attention':<16}{r['shape']:>42}{'':>4}{r['us']:>9.1f}{r['tflops']:>9.1f}"
+                         f"{r['hbm_bytes'] / 1e6:>8.1f} {r['bound']:<7}{100 * r['share']:>6.2f}%")
         else:
             lines.append(f"{'':>4} {r['module']:<16}{r['kernel'][-40:]:>31}{'':>4}{r['us']:>9.1f}{'':>26}{100 * r['share']:>6.2f}%")
     with open(os.path.join(args.out, "profile.txt"), "w") as f:
