@@ -107,7 +107,26 @@ typedef struct ladi_conv_desc {
    * 4/9 of the multiply-adds of the materialised form and no intermediate tensor.  ksize 3, stride 1, bf16 output. */
   int up2x;
 } ladi_conv_desc;
+/* Placement rules (LADI_ERR_INVALID, naming the operand, when broken): sources and shortcuts 16-byte aligned with pitches that are
+ * multiples of 8; bf16 out and residual 4-byte aligned, fp32 out 8-byte aligned; out_pitch >= the output width (c_out, c_out/2 for
+ * GEGLU), residual_pitch >= c_out; rowstat_out 8-byte and ln_stats 16-byte aligned.
+ * Store paths, chosen per call from the descriptor (ladi_conv2d_plan names the one a call takes):
+ *  - staged (16-byte stores through shared memory): bf16 out, N tile <= 128, no pair / split-K / LayerNorm fold / row statistics,
+ *    c_out, output width and out_pitch multiples of 8, out 16-byte aligned, residual 16-byte aligned with residual_pitch % 8 == 0,
+ *    a per-column bias 8-byte aligned with an even bias_step_stride;
+ *  - split-K (fp32 partials in splitk_ws, then a reduce pass): only when c_out, out_pitch and residual_pitch are multiples of 4, out
+ *    and residual 8-byte aligned, bias 16-byte aligned with bias_step_stride % 4 == 0 and splitk_ws 16-byte aligned; otherwise the
+ *    call runs unsplit, which is not an error;
+ *  - fragment (stores from the accumulator): every other valid descriptor. */
 LADI_API int ladi_conv2d_bf16(const ladi_conv_desc* d, void* stream);
+/* The plan ladi_conv2d_bf16 would run for `d` on a device with `sms` SMs (sms <= 0: the current device's count): N tile, split-K
+ * factor and K blocks per split, CTA pairs (the cluster count is the launch's, from the occupancy API), staged epilogue, pipeline
+ * stages, tile grid and total K blocks.  The same validation and decision code as the launch; it dereferences no pointer and needs no
+ * device, so it also answers on a machine without a GPU. */
+typedef struct ladi_conv_plan {
+  int bn, splits, kb_per_split, pair, staged, stages, tiles_m, tiles_n, total_kb;
+} ladi_conv_plan;
+LADI_API int ladi_conv2d_plan(const ladi_conv_desc* d, int sms, ladi_conv_plan* out);
 
 /* ---- fused multi-head attention, head_dim 64 (flash-style: S and O live in registers, online softmax in exp2) -------
  * Replaces diffusers CrossAttention.forward for attn1 (self) and attn2 (cross, 77 text tokens) of every
@@ -124,6 +143,8 @@ typedef struct ladi_attn_desc {
   void* trace;               /* unused (NULL) */
   int head_dim;              /* ladi_attention_d512_bf16 only: 0 or 512 (the VAE), or 256 (reduced-width test models) */
 } ladi_attn_desc;
+/* Placement rules of both attention entry points (LADI_ERR_INVALID when broken): q, k, v 16-byte aligned, every pitch a multiple of 8
+ * and >= the head columns (heads*64, or head_dim), out 4-byte aligned (it is stored as bf16 pairs) with an even out_batch_stride. */
 LADI_API int ladi_attention_bf16(const ladi_attn_desc* d, void* stream);
 /* The same for ONE head of width 512: the VAE mid-block AttentionBlock (src/models/vae.py:81-90,112 encoder; :142-150,187 decoder;
  * N = h*w tokens: 3072 at 512x384, 12288 at 1024x768).  heads must be 1, pitches >= head_dim; `variant` / `trace` ignored.  Flash-style:

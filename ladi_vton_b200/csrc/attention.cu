@@ -517,6 +517,13 @@ int launch(const ladi_attn_desc* d, int cols, dim3 grid, cudaStream_t stream) {
   return LADI_OK;
 }
 
+// Both kernels store the output as bf16 pairs (4 bytes): out must be 4-byte aligned and every batch's rows start on a pair.
+int check_out_placement(const ladi_attn_desc* d) {
+  LADI_CHECK((reinterpret_cast<uintptr_t>(d->out) & 3) == 0, "out %p must be 4-byte aligned", d->out);
+  LADI_CHECK(d->out_batch_stride % 2 == 0, "out_batch_stride %lld must be even", (long long)d->out_batch_stride);
+  return LADI_OK;
+}
+
 }  // namespace
 
 extern "C" int ladi_attention_bf16(const ladi_attn_desc* d, void* stream_) {
@@ -524,7 +531,9 @@ extern "C" int ladi_attention_bf16(const ladi_attn_desc* d, void* stream_) {
   LADI_CHECK(d != nullptr && d->q && d->k && d->v && d->out, "null attention operand");
   LADI_CHECK(d->batch > 0 && d->heads > 0 && d->nq > 0 && d->nkv > 0, "bad attention extent");
   LADI_CHECK(d->q_pitch % 8 == 0 && d->k_pitch % 8 == 0 && d->v_pitch % 8 == 0 && d->out_pitch % 8 == 0, "pitches must be multiples of 8");
-  LADI_CHECK(d->q_pitch >= d->heads * 64 && d->k_pitch >= d->heads * 64 && d->v_pitch >= d->heads * 64, "pitch < heads*64");
+  LADI_CHECK(d->q_pitch >= d->heads * 64 && d->k_pitch >= d->heads * 64 && d->v_pitch >= d->heads * 64 && d->out_pitch >= d->heads * 64,
+             "pitch < heads*64");
+  if (const int rc = check_out_placement(d)) return rc;
   LADI_CHECK(d->variant == 0 || d->variant == 1 || d->variant == 2 || d->variant == 4 || d->variant == 5 || d->variant == 6 ||
                  (d->variant == 8 && d->nkv <= 128),
              "bad attention variant %d", d->variant);
@@ -560,6 +569,7 @@ extern "C" int ladi_attention_d512_bf16(const ladi_attn_desc* d, void* stream_) 
   const int D5 = d->head_dim == 0 ? 512 : d->head_dim;
   LADI_CHECK(D5 == 512 || D5 == 256, "wide attention: head_dim must be 512 (or 256), got %d", D5);
   LADI_CHECK(d->q_pitch >= D5 && d->k_pitch >= D5 && d->v_pitch >= D5 && d->out_pitch >= D5, "pitch < head_dim");
+  if (const int rc = check_out_placement(d)) return rc;
   const dim3 grid((d->nq + BQ - 1) / BQ, D5 / 128, d->batch);
   return D5 == 512 ? launch<512>(d, D5, grid, stream) : launch<256>(d, D5, grid, stream);
 }

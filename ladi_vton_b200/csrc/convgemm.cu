@@ -577,8 +577,17 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restr
 constexpr size_t SMEM_LIMIT = 232448;  // 227 KiB per CTA
 constexpr size_t SMEM_TAIL = 2 * MAX_STAGES * 8 + 1024;  // barriers + alignment slack
 
+// Pipeline depth of an N tile and store path: as many (A, B) stages as fit beside the staging tile, at most MAX_STAGES.
+int pipeline_stages(int bn, bool staged) {
+  const size_t per_stage = A_BYTES + (size_t)bn * BK * 2;
+  const size_t staging = staged ? (size_t)BM * bn * 2 + STAGE_ROWTAB_BYTES : 0;
+  const int stages = (int)((SMEM_LIMIT - SMEM_TAIL - staging) / per_stage);
+  return stages > MAX_STAGES ? MAX_STAGES : stages;
+}
+
+// kp.stages is the plan's (pipeline_stages); the launch sizes shared memory and the grid from it and the tile grid.
 template <int BN, bool PAIR>
-int launch(const AMaps& am, const CUtensorMap& tmB, KParams& kp, cudaStream_t stream) {
+int launch(const AMaps& am, const CUtensorMap& tmB, const KParams& kp, cudaStream_t stream) {
   static bool attr_set = false;
   static int max_clusters = 0;
   if (!attr_set) {
@@ -599,11 +608,7 @@ int launch(const AMaps& am, const CUtensorMap& tmB, KParams& kp, cudaStream_t st
   }
   const size_t per_stage = A_BYTES + (size_t)BN * BK * 2;
   const size_t staging = kp.staged ? (size_t)BM * BN * 2 + STAGE_ROWTAB_BYTES : 0;
-  int stages = (int)((SMEM_LIMIT - SMEM_TAIL - staging) / per_stage);
-  if (stages > MAX_STAGES) stages = MAX_STAGES;
-  LADI_CHECK(stages >= 2, "not enough shared memory for a 2-stage pipeline");
-  kp.stages = stages;
-  const size_t smem = staging + stages * per_stage + SMEM_TAIL;
+  const size_t smem = staging + kp.stages * per_stage + SMEM_TAIL;
   if (PAIR) {
     const int items = ((kp.tiles_m + 1) / 2) * kp.tiles_n;
     const int clusters = items < max_clusters ? items : max_clusters;
@@ -643,6 +648,16 @@ int validate(const ladi_conv_desc* d) {
   LADI_CHECK(d->ln_stats == nullptr || (d->ln_colsum != nullptr && d->c_out % 32 == 0 && d->ksize == 1 && d->n_src == 1 && d->n_sc == 0 &&
                                         d->src_c[0] % 64 == 0 && !d->out_fp32 && !d->bias_per_row && !up),
              "ln_stats: GEMM over one source of K %% 64 == 0, c_out %% 32 == 0, bf16 out, ln_colsum given");
+  // placements no store path can serve (the fragment path stores bf16 pairs as 4 bytes, fp32 pairs as 8, reads residual pairs as 4,
+  // writes row statistics as float2 and reads them as float4); the staged and split-K paths need more and are chosen only when it holds
+  auto misaligned = [](const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; };
+  LADI_CHECK(!misaligned(d->out, d->out_fp32 ? 8 : 4), "out %p: %s output must be %d-byte aligned", d->out, d->out_fp32 ? "fp32" : "bf16",
+             d->out_fp32 ? 8 : 4);
+  LADI_CHECK(d->out_pitch >= (d->act == 2 ? d->c_out / 2 : d->c_out), "out_pitch %d below the output width", d->out_pitch);
+  LADI_CHECK(d->residual == nullptr || !misaligned(d->residual, 4), "residual %p must be 4-byte aligned", d->residual);
+  LADI_CHECK(d->residual == nullptr || d->residual_pitch >= d->c_out, "residual_pitch %d below c_out %d", d->residual_pitch, d->c_out);
+  LADI_CHECK(d->rowstat_out == nullptr || !misaligned(d->rowstat_out, 8), "rowstat_out %p must be 8-byte aligned", (void*)d->rowstat_out);
+  LADI_CHECK(d->ln_stats == nullptr || !misaligned(d->ln_stats, 16), "ln_stats %p must be 16-byte aligned", (const void*)d->ln_stats);
   return LADI_OK;
 }
 
@@ -664,39 +679,29 @@ void tile_geometry(const ladi_conv_desc* d, KParams& kp) {
   if (up) kp.tiles_m *= 4;
 }
 
-// A tensor maps, one per (source, parity plane) and per shortcut source, and the K segments that walk them: taps (row-major) x
-// sources, then the shortcut sources.  Weight K order must match (see packer).
-int build_a_maps_and_segments(const ladi_conv_desc* d, KParams& kp, AMaps& am) {
+// The input extent the A tensor maps cover (up2x: the half-resolution input = one output parity plane).
+int input_h(const ladi_conv_desc* d, const KParams& kp) { return kp.up2x ? kp.H : (d->h_in > 0 ? d->h_in : d->h_out * d->stride); }
+int input_w(const ladi_conv_desc* d, const KParams& kp) { return kp.up2x ? kp.W : (d->w_in > 0 ? d->w_in : d->w_out * d->stride); }
+
+// The K segments (host arithmetic only): taps (row-major) x sources, then the shortcut sources; weight K order must match (see packer).
+// A tensor maps are numbered as encode_a_maps writes them: the stride x stride parity planes of each source, then one per shortcut.
+int walk_segments(const ladi_conv_desc* d, KParams& kp) {
   const int up = kp.up2x, s = d->stride;
-  const int h_in = up ? kp.H : (d->h_in > 0 ? d->h_in : d->h_out * s), w_in = up ? kp.W : (d->w_in > 0 ? d->w_in : d->w_out * s);
-  const uint32_t box[4] = {(uint32_t)BK, (uint32_t)kp.bw, (uint32_t)kp.bh, (uint32_t)kp.bn};
   int nmaps = 0, src_map0[2] = {0, 0}, sc_map0[2] = {0, 0};
-  // the st x st parity planes of one NHWC tensor (st = 1: the tensor itself)
-  auto add_maps = [&](const void* ptr, int c, int pitch_, int w, int h, int st) -> int {
-    for (int py = 0; py < st; ++py)
-      for (int px = 0; px < st; ++px) {
-        LADI_CHECK(nmaps < NUM_A_MAPS, "too many tensor maps");
-        const uint64_t pitch = (uint64_t)pitch_;
-        const uint64_t dims[4] = {(uint64_t)c, (uint64_t)((w - px + st - 1) / st), (uint64_t)((h - py + st - 1) / st), (uint64_t)d->n};
-        const uint64_t strides[3] = {pitch * 2 * st, pitch * 2 * w * st, pitch * 2 * (uint64_t)w * h};
-        const bf16* base = reinterpret_cast<const bf16*>(ptr) + ((size_t)py * w + px) * pitch;
-        if (ladi_encode_tmap_bf16(&am.m[nmaps++], base, 4, dims, strides, box)) return LADI_ERR_CUDA;
-      }
-    return LADI_OK;
-  };
   for (int i = 0; i < d->n_src; ++i) {
-    LADI_CHECK(d->src[i] != nullptr && d->src_c[i] > 0 && d->src_pitch[i] % 8 == 0 && d->src_pitch[i] >= d->src_c[i],
-               "source %d: need non-null, pitch multiple of 8 and >= C", i);
+    LADI_CHECK(d->src[i] != nullptr && d->src_c[i] > 0 && d->src_pitch[i] % 8 == 0 && d->src_pitch[i] >= d->src_c[i] &&
+                   reinterpret_cast<uintptr_t>(d->src[i]) % 16 == 0,
+               "source %d: need non-null and 16-byte aligned, pitch multiple of 8 and >= C", i);
     src_map0[i] = nmaps;
-    if (const int rc = add_maps(d->src[i], d->src_c[i], d->src_pitch[i], w_in, h_in, s)) return rc;
+    nmaps += s * s;
   }
   for (int i = 0; i < d->n_sc; ++i) {
     LADI_CHECK(s == 1, "fused 1x1 shortcut requires stride 1");
-    LADI_CHECK(d->sc[i] != nullptr && d->sc_c[i] > 0 && d->sc_pitch[i] % 8 == 0, "shortcut source %d invalid", i);
-    sc_map0[i] = nmaps;
-    if (const int rc = add_maps(d->sc[i], d->sc_c[i], d->sc_pitch[i], d->w_out, d->h_out, 1)) return rc;
+    LADI_CHECK(d->sc[i] != nullptr && d->sc_c[i] > 0 && d->sc_pitch[i] % 8 == 0 && reinterpret_cast<uintptr_t>(d->sc[i]) % 16 == 0,
+               "shortcut source %d invalid", i);
+    sc_map0[i] = nmaps++;
   }
-  for (int i = nmaps; i < NUM_A_MAPS; ++i) am.m[i] = am.m[0];
+  LADI_CHECK(nmaps <= NUM_A_MAPS, "too many tensor maps");
 
   int nseg = 0, total = 0;
   auto add_seg = [&](int map, int dx, int dy, int channels) -> int {
@@ -726,6 +731,31 @@ int build_a_maps_and_segments(const ladi_conv_desc* d, KParams& kp, AMaps& am) {
   return LADI_OK;
 }
 
+// The A tensor maps walk_segments numbered: one per (source, parity plane), then one per shortcut source.
+int encode_a_maps(const ladi_conv_desc* d, const KParams& kp, AMaps& am) {
+  const int s = d->stride, h_in = input_h(d, kp), w_in = input_w(d, kp);
+  const uint32_t box[4] = {(uint32_t)BK, (uint32_t)kp.bw, (uint32_t)kp.bh, (uint32_t)kp.bn};
+  int nmaps = 0;
+  // the st x st parity planes of one NHWC tensor (st = 1: the tensor itself)
+  auto add_maps = [&](const void* ptr, int c, int pitch_, int w, int h, int st) -> int {
+    for (int py = 0; py < st; ++py)
+      for (int px = 0; px < st; ++px) {
+        const uint64_t pitch = (uint64_t)pitch_;
+        const uint64_t dims[4] = {(uint64_t)c, (uint64_t)((w - px + st - 1) / st), (uint64_t)((h - py + st - 1) / st), (uint64_t)d->n};
+        const uint64_t strides[3] = {pitch * 2 * st, pitch * 2 * w * st, pitch * 2 * (uint64_t)w * h};
+        const bf16* base = reinterpret_cast<const bf16*>(ptr) + ((size_t)py * w + px) * pitch;
+        if (const int rc = ladi_encode_tmap_bf16(&am.m[nmaps++], base, 4, dims, strides, box)) return rc;
+      }
+    return LADI_OK;
+  };
+  for (int i = 0; i < d->n_src; ++i)
+    if (const int rc = add_maps(d->src[i], d->src_c[i], d->src_pitch[i], w_in, h_in, s)) return rc;
+  for (int i = 0; i < d->n_sc; ++i)
+    if (const int rc = add_maps(d->sc[i], d->sc_c[i], d->sc_pitch[i], d->w_out, d->h_out, 1)) return rc;
+  for (int i = nmaps; i < NUM_A_MAPS; ++i) am.m[i] = am.m[0];
+  return LADI_OK;
+}
+
 // The path one descriptor takes: the ONLY place that decides it.  Reads nothing but its arguments.
 struct Plan {
   int bn, splits, kb_per_split;  // N tile; split-K (splits > 1: fp32 partials, splitk_reduce_kernel runs the epilogue), as in KParams
@@ -739,9 +769,14 @@ Plan choose_plan(const ladi_conv_desc* d, int tiles_m, int total_kb, int sms) {
   if (d->force_bn > 0) pl.bn = d->force_bn;
   // 2. split-K: few output tiles but a long reduction (the 8x6 / 16x12 UNet levels): spread K over otherwise idle SMs, fp32 partial
   // planes in the caller's workspace, summed (in split order) by splitk_reduce_kernel.  Its N tile is the widest that c_out fills.
+  // The reduce moves 4 columns at a time (float4 workspace and bias loads, 8-byte residual loads and output stores): a placement
+  // without that alignment runs unsplit.
+  const auto aligned = [](const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; };
   if (d->splitk_ws != nullptr && d->force_bn == 0 && !d->out_fp32 && d->act != 2 && d->row_scale == nullptr && !d->bias_per_row && !up &&
       d->rowstat_out == nullptr && d->ln_stats == nullptr &&
-      d->c_out % 4 == 0 && d->out_pitch % 4 == 0 && (d->residual == nullptr || d->residual_pitch % 4 == 0) && total_kb >= 32) {
+      d->c_out % 4 == 0 && d->out_pitch % 4 == 0 && (d->residual == nullptr || d->residual_pitch % 4 == 0) && total_kb >= 32 &&
+      aligned(d->out, 8) && aligned(d->residual, 8) && aligned(d->splitk_ws, 16) &&
+      (d->bias == nullptr || (aligned(d->bias, 16) && d->bias_step_stride % 4 == 0))) {
     const int bn_s = d->c_out >= 256 ? 256 : (d->c_out >= 128 ? 128 : 64);
     const long tiles_s = (long)tiles_m * ((d->c_out + bn_s - 1) / bn_s);
     if (tiles_s * 2 <= sms) {
@@ -801,8 +836,8 @@ int encode_b_map(const ladi_conv_desc* d, const Plan& pl, CUtensorMap* tmB) {
 }
 
 // The kernel of the plan's (BN, pair), then the split-K second pass with the descriptor's own epilogue operands.
-int launch_plan(const ladi_conv_desc* d, const Plan& pl, const AMaps& am, const CUtensorMap& tmB, KParams& kp, cudaStream_t stream) {
-  using Launch = int (*)(const AMaps&, const CUtensorMap&, KParams&, cudaStream_t);
+int launch_plan(const ladi_conv_desc* d, const Plan& pl, const AMaps& am, const CUtensorMap& tmB, const KParams& kp, cudaStream_t stream) {
+  using Launch = int (*)(const AMaps&, const CUtensorMap&, const KParams&, cudaStream_t);
   static const struct { int bn; Launch single, pair; } table[6] = {  // every instantiation there is; tiles below 128 do not pair
       {256, launch<256, false>, launch<256, true>}, {192, launch<192, false>, launch<192, true>},
       {160, launch<160, false>, launch<160, true>}, {128, launch<128, false>, launch<128, true>},
@@ -822,21 +857,41 @@ int launch_plan(const ladi_conv_desc* d, const Plan& pl, const AMaps& am, const 
   return LADI_OK;
 }
 
-}  // namespace
-
-extern "C" int ladi_conv2d_bf16(const ladi_conv_desc* d, void* stream_) {
+// Everything a launch decides, from the descriptor and the SM count alone (no pointer is dereferenced, nothing touches a device):
+// validation, tile grid, K segments, the plan (choose_plan) and the pipeline depth.  ladi_conv2d_plan reports it; ladi_conv2d_bf16
+// launches it.
+int plan_conv(const ladi_conv_desc* d, int sms, KParams& kp, Plan& pl) {
   if (const int rc = validate(d)) return rc;
-  KParams kp;
   memset(&kp, 0, sizeof(kp));
-  AMaps am;
   tile_geometry(d, kp);
-  if (const int rc = build_a_maps_and_segments(d, kp, am)) return rc;
-  const Plan pl = choose_plan(d, kp.tiles_m, kp.total_kb, ladi_num_sms());
+  if (const int rc = walk_segments(d, kp)) return rc;
+  pl = choose_plan(d, kp.tiles_m, kp.total_kb, sms);
   LADI_CHECK(d->pair_mode != 1 || pl.pair, "pair_mode=1 needs >= 2 M tiles, BN >= 128 and no split-K (BN=%d, tiles_m=%d)", pl.bn, kp.tiles_m);
-
-  // ---- the plan and the descriptor's epilogue operands -> kernel parameters
   kp.tiles_n = (d->c_out + pl.bn - 1) / pl.bn;
   kp.splits = pl.splits; kp.kb_per_split = pl.kb_per_split; kp.staged = pl.staged; kp.form = pl.form;
+  kp.stages = pipeline_stages(pl.bn, pl.staged);
+  LADI_CHECK(kp.stages >= 2, "not enough shared memory for a 2-stage pipeline");
+  return LADI_OK;
+}
+
+}  // namespace
+
+extern "C" int ladi_conv2d_plan(const ladi_conv_desc* d, int sms, ladi_conv_plan* out) {
+  LADI_CHECK(out != nullptr, "plan output is null");
+  KParams kp;
+  Plan pl;
+  if (const int rc = plan_conv(d, sms > 0 ? sms : ladi_num_sms(), kp, pl)) return rc;
+  out->bn = pl.bn; out->splits = pl.splits; out->kb_per_split = pl.kb_per_split; out->pair = pl.pair; out->staged = pl.staged;
+  out->stages = kp.stages; out->tiles_m = kp.tiles_m; out->tiles_n = kp.tiles_n; out->total_kb = kp.total_kb;
+  return LADI_OK;
+}
+
+extern "C" int ladi_conv2d_bf16(const ladi_conv_desc* d, void* stream_) {
+  KParams kp;
+  Plan pl;
+  if (const int rc = plan_conv(d, ladi_num_sms(), kp, pl)) return rc;
+
+  // ---- the descriptor's epilogue operands -> kernel parameters
   kp.bias = d->bias; kp.bias_per_row = d->bias_per_row; kp.bias_step_stride = d->bias_step_stride; kp.step_ptr = d->step_ptr;
   kp.residual = reinterpret_cast<const bf16*>(d->residual); kp.residual_pitch = d->residual_pitch;
   kp.row_scale = d->row_scale; kp.act = d->act; kp.out = d->out; kp.out_pitch = d->out_pitch; kp.out_fp32 = d->out_fp32;
@@ -847,6 +902,8 @@ extern "C" int ladi_conv2d_bf16(const ladi_conv_desc* d, void* stream_) {
     kp.out = d->splitk_ws; kp.out_pitch = d->c_out; kp.out_fp32 = 1;
     kp.bias = nullptr; kp.step_ptr = nullptr; kp.act = 0; kp.residual = nullptr;
   }
+  AMaps am;
+  if (const int rc = encode_a_maps(d, kp, am)) return rc;
   CUtensorMap tmB;
   if (const int rc = encode_b_map(d, pl, &tmB)) return rc;
   return launch_plan(d, pl, am, tmB, kp, reinterpret_cast<cudaStream_t>(stream_));

@@ -28,6 +28,14 @@ class ConvDesc(C.Structure):
     ]
 
 
+class ConvPlan(C.Structure):  # ladi_conv_plan: the path ladi_conv2d_bf16 takes for a descriptor (ladi_conv2d_plan)
+    _fields_ = [(f, C.c_int) for f in ("bn", "splits", "kb_per_split", "pair", "staged", "stages", "tiles_m", "tiles_n", "total_kb")]
+
+    def items(self):
+        """Work items of the persistent grid: (tile, K split) per CTA, or (pair of M tiles, N tile) per CTA pair."""
+        return (self.tiles_m + 1) // 2 * self.tiles_n if self.pair else self.tiles_m * self.tiles_n * self.splits
+
+
 class AttnDesc(C.Structure):
     _fields_ = [
         ("batch", C.c_int), ("heads", C.c_int), ("nq", C.c_int), ("nkv", C.c_int),
@@ -63,6 +71,7 @@ SIGNATURES = {
     "ladi_last_error": ([], C.c_char_p),
     "ladi_launch_count": ([], C.c_longlong),
     "ladi_conv2d_bf16": ([C.POINTER(ConvDesc), _P], _I),
+    "ladi_conv2d_plan": ([C.POINTER(ConvDesc), _I, C.POINTER(ConvPlan)], _I),
     "ladi_attention_bf16": ([C.POINTER(AttnDesc), _P], _I),
     "ladi_attention_d512_bf16": ([C.POINTER(AttnDesc), _P], _I),
     "ladi_groupnorm_chunks": ([_I], _I),
@@ -160,3 +169,12 @@ def call(name, *args):
         raise RuntimeError(f"{name} failed ({rc}): {lib.ladi_last_error().decode()}")
     launches += lib.ladi_launch_count() - before
     return rc
+
+
+def conv_plan(desc, sms=0):
+    """The plan ladi_conv2d_bf16 runs for `desc` on `sms` SMs (0: this device's); launches nothing.  Invalid -> RuntimeError."""
+    plan = ConvPlan()
+    lib = load()
+    if lib.ladi_conv2d_plan(C.byref(desc), sms, C.byref(plan)) != 0:
+        raise RuntimeError(f"ladi_conv2d_plan failed: {lib.ladi_last_error().decode()}")
+    return plan

@@ -65,22 +65,36 @@ def padded_k(channels):
     return (channels + BK - 1) // BK * BK
 
 
-def conv2d(srcs, weight, c_out, *, ksize=3, stride=1, pad_lo=1, shortcut=(), bias=None, bias_per_row=False,
-           bias_step_stride=0, step_ptr=None, residual=None, row_scale=None, act=ACT_NONE, out=None, out_fp32=False,
-           force_bn=0, direct_epilogue=False, split_k=True, pair=None, rowstat=None, ln=None, up2x=False):
+def conv2d(srcs, weight, c_out, **kw):
     """Implicit-GEMM convolution over the channel-concat of `srcs` (+ fused 1x1 over `shortcut` tensors).
     `weight`: packed bf16 [c_out, k_total] (see weights.pack_conv).  Returns the NHWC output tensor.
     rowstat: fp32 [rows, c_out/32, 2] table this call fills with per-row partial {sum, sum of squares} (LayerNorm producer side);
     ln = (stats table of the A rows, colsum fp32 [c_out], eps): LayerNorm folded into this GEMM (weights.fold_layernorm);
     up2x: `srcs` are half-resolution, `weight` = weights.pack_conv_up2x (nearest-2x upsample fused into the 3x3 conv)."""
+    d, out, flops, tag = _conv_desc(srcs, weight, c_out, **kw)
+    _call("ladi_conv2d_bf16", flops, C.byref(d), _stream(), tag=tag)
+    return out
+
+
+def conv_plan(srcs, weight, c_out, sms=0, **kw):
+    """The plan (lib.ConvPlan: N tile, split-K, pair, store path, stages, tile grid) conv2d(srcs, weight, c_out, **kw) runs on a device
+    with `sms` SMs (0: this one's); launches nothing."""
+    return lib.conv_plan(_conv_desc(srcs, weight, c_out, **kw)[0], sms)
+
+
+def _conv_desc(srcs, weight, c_out, *, ksize=3, stride=1, pad_lo=1, shortcut=(), bias=None, bias_per_row=False,
+               bias_step_stride=0, step_ptr=None, residual=None, row_scale=None, act=ACT_NONE, out=None, out_fp32=False,
+               force_bn=0, direct_epilogue=False, split_k=True, pair=None, rowstat=None, ln=None, up2x=False):
+    """-> (ConvDesc, output tensor, algorithmic flops, profile tag) of one conv2d call."""
     assert 1 <= len(srcs) <= 2 and len(shortcut) <= 2
     d = ConvDesc()
     n, h_in, w_in, _, _ = _nhwc(srcs[0])
     if up2x:
         assert ksize == 3 and stride == 1
         h_out, w_out = 2 * h_in, 2 * w_in
-    elif ksize == 3 and stride == 2:
-        h_out, w_out = (h_in + (2 if pad_lo == 1 else 1) - 3) // 2 + 1, (w_in + (2 if pad_lo == 1 else 1) - 3) // 2 + 1
+    elif stride == 2:  # 3x3: padding pad_lo before, 1 after (the VAE's (0, 1, 0, 1) downsample: 0 before); 1x1: none
+        pads = (2 if pad_lo == 1 else 1) if ksize == 3 else 0
+        h_out, w_out = (h_in + pads - ksize) // 2 + 1, (w_in + pads - ksize) // 2 + 1
     else:
         h_out, w_out = h_in, w_in
     d.n, d.h_out, d.w_out, d.c_out = n, h_out, w_out, c_out
@@ -136,23 +150,33 @@ def conv2d(srcs, weight, c_out, *, ksize=3, stride=1, pad_lo=1, shortcut=(), bia
     # algorithmic flops: 2 * output pixels * c_out * true reduction length (padding channels excluded)
     # (a fused-upsample conv is credited with the 9 taps of the convolution it replaces: algorithmic work is implementation independent)
     k_true = ksize * ksize * sum(int(t.shape[3]) for t in srcs) + sum(int(t.shape[3]) for t in shortcut)
-    _call("ladi_conv2d_bf16", 2.0 * n * h_out * w_out * c_out * k_true, C.byref(d), _stream(),
-          tag=f"k{ksize}s{stride}{'u' if up2x else ''} M={n * h_out * w_out} N={c_out} K={k_true} act={act}{' ln' if ln is not None else ''}{' rs' if rowstat is not None else ''}")
-    return out
+    return (d, out, 2.0 * n * h_out * w_out * c_out * k_true,
+            f"k{ksize}s{stride}{'u' if up2x else ''} M={n * h_out * w_out} N={c_out} K={k_true} act={act}{' ln' if ln is not None else ''}{' rs' if rowstat is not None else ''}")
+
+
+def _gemm_views(a, kw):
+    """a [M, K] (row-strided) and the out / residual of kw as the 1 x 1 x M images conv2d takes."""
+    assert a.dim() == 2 and a.stride(1) == 1
+    a4 = a.as_strided((1, 1, a.shape[0], a.shape[1]), (a.stride(0) * a.shape[0], a.stride(0) * a.shape[0], a.stride(0), 1))
+    kw = dict(kw)
+    for key in ("out", "residual"):
+        t = kw.get(key)
+        if t is not None:
+            kw[key] = t.as_strided((1, 1, t.shape[0], t.shape[1]), (0, 0, t.stride(0), 1))
+    return a4, kw
 
 
 def gemm(a, weight, n_out, **kw):
     """out[M, n_out] = epilogue(a[M, K] @ weight[n_out, K]^T); `a` may be a row-strided 2-D view."""
-    assert a.dim() == 2 and a.stride(1) == 1
-    a4 = a.as_strided((1, 1, a.shape[0], a.shape[1]), (a.stride(0) * a.shape[0], a.stride(0) * a.shape[0], a.stride(0), 1))
-    out = kw.pop("out", None)
-    res = kw.pop("residual", None)
-    if out is not None:
-        out = out.as_strided((1, 1, out.shape[0], out.shape[1]), (0, 0, out.stride(0), 1))
-    if res is not None:
-        res = res.as_strided((1, 1, res.shape[0], res.shape[1]), (0, 0, res.stride(0), 1))
-    o = conv2d([a4], weight, n_out, ksize=1, out=out, residual=res, **kw)
+    a4, kw = _gemm_views(a, kw)
+    o = conv2d([a4], weight, n_out, ksize=1, **kw)
     return o[0, 0]
+
+
+def gemm_plan(a, weight, n_out, sms=0, **kw):
+    """The plan gemm(a, weight, n_out, **kw) runs (see conv_plan)."""
+    a4, kw = _gemm_views(a, kw)
+    return conv_plan([a4], weight, n_out, sms=sms, ksize=1, **kw)
 
 
 def attention(q, k, v, heads, scale, out=None, variant=0, trace=None):

@@ -59,16 +59,19 @@ def _padded(rows, c, pitch, dev, fill=None):
 
 
 def _run_both(call, form, rows, c_eff, res, dev):
-    """call(out [rows, pitch] view, residual view or None) for a staged pitch (c_eff + 8) and a fragment pitch (c_eff + 4)."""
+    """call(out [rows, pitch] view, residual view or None, plan=False) for a staged pitch (c_eff + 8) and a fragment pitch (c_eff + 4);
+    call(..., plan=True) returns the plan (ladi_conv2d_plan) of the same call, which must be the staged one and the fragment one."""
     outs = []
-    for pitch in (c_eff + 8, c_eff + 4):
+    for pitch, staged in ((c_eff + 8, 1), (c_eff + 4, 0)):
         if form == "inplace":
             buf = _padded(rows, c_eff, pitch, dev, res)
-            call(buf, buf[:, :c_eff])
+            rbuf = buf[:, :c_eff]
         else:
             buf = _padded(rows, c_eff, pitch, dev)
             rbuf = None if res is None else _padded(rows, c_eff, pitch, dev, res)[:, :c_eff]
-            call(buf, rbuf)
+        plan = call(buf, rbuf, plan=True)
+        assert (plan.staged, plan.splits, plan.pair) == (staged, 1, 0), f"pitch {pitch}: staged {plan.staged}, want {staged}"
+        call(buf, rbuf)
         outs.append(buf)
     torch.cuda.synchronize()
     staged, frag = outs
@@ -109,8 +112,8 @@ def test_staged_gemm(cuda, form, bn):
     kw, bcol, brow, res, rs, act = _inputs(form, M, c_out, c_eff, cuda, 12)
     wp = weights.pack_linear(w.float())
 
-    def call(out, resid):
-        ops.gemm(a, wp, c_out, out=out[:, :c_eff], residual=resid, force_bn=bn, split_k=False, **kw)
+    def call(out, resid, plan=False):
+        return (ops.gemm_plan if plan else ops.gemm)(a, wp, c_out, out=out[:, :c_eff], residual=resid, force_bn=bn, split_k=False, **kw)
 
     y = _run_both(call, form, M, c_eff, res, cuda)
     acc = a.double() @ w.double().t()
@@ -138,10 +141,11 @@ def test_staged_conv(cuda, form, shape):
     kw, bcol, brow, res, rs, act = _inputs(form, rows, c_out, c_out, cuda, 22)
     wp = weights.pack_conv_up2x(wt, [C]) if up else weights.pack_conv(wt, [C])
 
-    def call(out, resid):
+    def call(out, resid, plan=False):
         o4 = out.view(n, ho, wo, out.shape[1])[..., :c_out]
         r4 = None if resid is None else resid.view(n, ho, wo, c_out)
-        ops.conv2d([x], wp, c_out, ksize=3, out=o4, residual=r4, force_bn=128, split_k=False, up2x=up, **kw)
+        return (ops.conv_plan if plan else ops.conv2d)([x], wp, c_out, ksize=3, out=o4, residual=r4, force_bn=128, split_k=False, up2x=up,
+                                                       **kw)
 
     y = _run_both(call, form, rows, c_out, res, cuda)
     xd = x.double().permute(0, 3, 1, 2)
