@@ -163,9 +163,34 @@ LADI_API int ladi_groupnorm_stats(const void* x0, int c0, int pitch0, const void
 LADI_API int ladi_groupnorm_apply(const void* x0, int c0, int pitch0, const void* x1, int c1, int pitch1, int n, int hw, int groups,
                          const float* ws, const float* gamma, const float* beta, float eps, int silu, const void* add,
                          int add_pitch, void* out, int out_pitch, void* stream);
-/* LayerNorm over the last dim (BasicTransformerBlock.norm1/2/3; inversion adapter LayerNorms). */
+/* Placement rules (LADI_ERR_INVALID, naming the operand, when broken).  Both passes: x0 16-byte aligned, c0 > 0, c0 and pitch0
+ * multiples of 8 with pitch0 >= c0; c1 >= 0, and when c1 > 0 x1 16-byte aligned with c1 and pitch1 multiples of 8, pitch1 >= c1;
+ * n > 0, hw > 0; ws non-null; groups <= 64 dividing c0 + c1 <= 2560.  Apply also: gamma and beta non-null (read as scalars); out
+ * 16-byte aligned with out_pitch % 8 == 0 and >= c0 + c1; add (optional) 16-byte aligned with add_pitch % 8 == 0 and >= c0 + c1. */
+/* The grids the two passes launch for these arguments on a device with `sms` SMs (sms <= 0: the current device's count): pixel
+ * chunks per image; group splits (gsplit: blockIdx.z of the stats pass, each owning block_channels channels); the stats block's
+ * 16-byte channel lanes (lanes_v) and pixel lanes (k); pixels per chunk; the apply pass's pixels per block and block count; its
+ * cursor step of dp pixels plus dv vectors per 256 elements; the threads per group (slices) folding the chunk partials.  The same
+ * validation and decision code as the launches; it dereferences no pointer and needs no device. */
+typedef struct ladi_gn_plan {
+  int chunks, gsplit, block_channels, lanes_v, k, px_per_chunk, px_per_block, apply_blocks, dv, dp, slices;
+} ladi_gn_plan;
+LADI_API int ladi_groupnorm_plan(const void* x0, int c0, int pitch0, const void* x1, int c1, int pitch1, int n, int hw, int groups,
+                         const float* ws, const float* gamma, const float* beta, float eps, int silu, const void* add,
+                         int add_pitch, const void* out, int out_pitch, int sms, ladi_gn_plan* plan);
+/* LayerNorm over the last dim (BasicTransformerBlock.norm1/2/3; inversion adapter LayerNorms).  Two-pass statistics per row (mean,
+ * then the sum of squared deviations).  Placement rules (LADI_ERR_INVALID, naming the operand): x, out, gamma and beta 16-byte aligned;
+ * c a multiple of 8, <= 2048, with c / 8 = T * VPL for T in {4, 8, 16, 32} and VPL <= 8; x_pitch and out_pitch multiples of 8 and
+ * >= c; rows > 0. */
 LADI_API int ladi_layernorm(const void* x, int x_pitch, int rows, int c, const float* gamma, const float* beta, float eps, void* out,
                    int out_pitch, void* stream);
+/* The LayerNorm launch for these arguments: T lanes per row, VPL 16-byte vectors per lane, rows per 256-thread block, blocks.  `sms` is
+ * accepted like ladi_groupnorm_plan's; this plan does not depend on it.  Dereferences no pointer, needs no device. */
+typedef struct ladi_ln_plan {
+  int T, vpl, rows_per_block, blocks;
+} ladi_ln_plan;
+LADI_API int ladi_layernorm_plan(const void* x, int x_pitch, int rows, int c, const float* gamma, const float* beta, float eps,
+                         const void* out, int out_pitch, int sms, ladi_ln_plan* plan);
 /* Row softmax fp32 -> bf16 (VAE mid-block AttentionBlock: softmax in fp32, Appendix A.5). */
 LADI_API int ladi_softmax_rows(const float* s, int rows, int cols, int s_pitch, float scale, void* out, int out_pitch, void* stream);
 

@@ -628,40 +628,86 @@ inline int grid_for(int64_t total, int block = 256) {
 
 extern "C" int ladi_groupnorm_chunks(int hw) { return gn_chunks(hw); }
 
-static int gn_check(const void* x0, int c0, int pitch0, const void* x1, int c1, int pitch1, int groups) {
-  LADI_CHECK(x0 != nullptr && c0 > 0 && c0 % 8 == 0 && pitch0 % 8 == 0, "groupnorm source 0 invalid");
-  LADI_CHECK((x1 == nullptr && c1 == 0) || (x1 != nullptr && c1 % 8 == 0 && pitch1 % 8 == 0), "groupnorm source 1 invalid");
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// Everything the two GroupNorm launches decide, from their arguments and the SM count alone (no pointer is dereferenced, nothing touches
+// a device): validation, then the stats grid (pixel chunks x images x group splits) and the apply grid.  ladi_groupnorm_plan reports
+// it; ladi_groupnorm_stats / ladi_groupnorm_apply launch it.
+static int gn_plan_stats(const void* x0, int c0, int pitch0, const void* x1, int c1, int pitch1, int n, int hw, int groups,
+                         const void* ws, int sms, ladi_gn_plan& pl) {
+  LADI_CHECK(x0 != nullptr && c0 > 0 && c0 % 8 == 0 && pitch0 % 8 == 0 && pitch0 >= c0,
+             "groupnorm x0: need non-null, c0 > 0 and a multiple of 8, pitch0 a multiple of 8 and >= c0 (c0 %d, pitch0 %d)", c0, pitch0);
+  LADI_CHECK(aligned16(x0), "groupnorm x0 %p must be 16-byte aligned", x0);
+  LADI_CHECK(c1 >= 0 && ((x1 == nullptr && c1 == 0) || (x1 != nullptr && c1 % 8 == 0 && pitch1 % 8 == 0 && pitch1 >= c1)),
+             "groupnorm x1: need c1 >= 0 (0 when x1 is null) and a multiple of 8, pitch1 a multiple of 8 and >= c1 (c1 %d, pitch1 %d)",
+             c1, pitch1);
+  LADI_CHECK(c1 == 0 || aligned16(x1), "groupnorm x1 %p must be 16-byte aligned", x1);
+  LADI_CHECK(n > 0 && hw > 0, "groupnorm: need n > 0 and hw > 0 (n %d, hw %d)", n, hw);
+  LADI_CHECK(ws != nullptr, "groupnorm ws is null");
   LADI_CHECK(groups > 0 && groups <= GN_MAX_GROUPS && (c0 + c1) % groups == 0, "groupnorm: C %% groups != 0 or groups > 64");
   LADI_CHECK(c0 + c1 <= GN_SLOTS, "groupnorm: more than %d channels", GN_SLOTS);
+  const int C = c0 + c1;
+  pl.chunks = gn_chunks(hw);
+  // split the groups over blockIdx.z until the grid covers the GPU twice; each split must own whole groups and whole 16-byte vectors
+  int gsplit = 1;
+  while (gsplit < 16 && (long)pl.chunks * n * gsplit < 2L * sms && groups % (gsplit * 2) == 0 && (C / (gsplit * 2)) % 8 == 0) gsplit *= 2;
+  pl.gsplit = gsplit;
+  pl.block_channels = C / gsplit;  // gn_stats_kernel: C = gps * cpg, nv = C / 8, lanes_v, k, per
+  pl.lanes_v = pl.block_channels / 8 < 256 ? pl.block_channels / 8 : 256;
+  pl.k = 256 / pl.lanes_v;
+  pl.px_per_chunk = (hw + pl.chunks - 1) / pl.chunks;
   return LADI_OK;
+}
+
+static int gn_plan_apply(const void* x0, int c0, int pitch0, const void* x1, int c1, int pitch1, int n, int hw, int groups, const void* ws,
+                         const float* gamma, const float* beta, const void* add, int add_pitch, const void* out, int out_pitch, int sms,
+                         ladi_gn_plan& pl) {
+  if (int e = gn_plan_stats(x0, c0, pitch0, x1, c1, pitch1, n, hw, groups, ws, sms, pl)) return e;
+  const int C = c0 + c1;
+  LADI_CHECK(gamma != nullptr && beta != nullptr, "groupnorm gamma / beta is null");
+  LADI_CHECK(out != nullptr && aligned16(out), "groupnorm out %p must be non-null and 16-byte aligned", out);
+  LADI_CHECK(out_pitch % 8 == 0 && out_pitch >= C, "groupnorm out_pitch %d must be a multiple of 8 and >= C (%d)", out_pitch, C);
+  LADI_CHECK(add == nullptr || aligned16(add), "groupnorm add %p must be 16-byte aligned", add);
+  LADI_CHECK(add == nullptr || (add_pitch % 8 == 0 && add_pitch >= C), "groupnorm add_pitch %d must be a multiple of 8 and >= C (%d)",
+             add_pitch, C);
+  const int nv = C / 8;
+  int ppb = (256 * 16) / nv;  // >= 16 vectors per thread, and few enough blocks that the per-block channel table amortises
+  const int target_blocks = (sms * 3 + n - 1) / n;  // 3 resident blocks per SM (launch bounds): the whole grid is one wave
+  const int ppb2 = (hw + target_blocks - 1) / target_blocks;
+  if (ppb2 > ppb) ppb = ppb2;
+  if (ppb < 1) ppb = 1;
+  pl.px_per_block = ppb;
+  pl.apply_blocks = (hw + ppb - 1) / ppb;
+  pl.dv = 256 % nv;  // gn_apply_kernel's cursor step: dp pixels and dv vectors per 256 elements
+  pl.dp = 256 / nv;
+  pl.slices = 256 / groups < 8 ? 256 / groups : 8;
+  return LADI_OK;
+}
+
+extern "C" int ladi_groupnorm_plan(const void* x0, int c0, int pitch0, const void* x1, int c1, int pitch1, int n, int hw, int groups,
+                                   const float* ws, const float* gamma, const float* beta, float eps, int silu, const void* add,
+                                   int add_pitch, const void* out, int out_pitch, int sms, ladi_gn_plan* plan) {
+  (void)eps; (void)silu;
+  LADI_CHECK(plan != nullptr, "plan output is null");
+  return gn_plan_apply(x0, c0, pitch0, x1, c1, pitch1, n, hw, groups, ws, gamma, beta, add, add_pitch, out, out_pitch,
+                       sms > 0 ? sms : ladi_num_sms(), *plan);
 }
 
 extern "C" int ladi_groupnorm_stats(const void* x0, int c0, int pitch0, const void* x1, int c1, int pitch1, int n, int hw, int groups,
                                     float* ws, void* stream) {
-  if (int e = gn_check(x0, c0, pitch0, x1, c1, pitch1, groups)) return e;
-  const int chunks = gn_chunks(hw);
-  // split the groups over blockIdx.z until the grid covers the GPU twice; each split must own whole groups and whole 16-byte vectors
-  int gsplit = 1;
-  while (gsplit < 16 && (long)chunks * n * gsplit < 2L * ladi_num_sms() && groups % (gsplit * 2) == 0 &&
-         ((c0 + c1) / (gsplit * 2)) % 8 == 0 && (c0 % ((c0 + c1) / (gsplit * 2)) == 0 || c1 == 0 || true))
-    gsplit *= 2;
-  LADI_CUDA(ladi_launch(gn_stats_kernel, dim3(dim3(chunks, n, gsplit)), dim3(256), 0, STREAM, (const bf16*)x0, c0, pitch0, (const bf16*)x1, c1, pitch1, hw, groups, chunks, ws));
+  ladi_gn_plan pl;
+  if (int e = gn_plan_stats(x0, c0, pitch0, x1, c1, pitch1, n, hw, groups, ws, ladi_num_sms(), pl)) return e;
+  LADI_CUDA(ladi_launch(gn_stats_kernel, dim3(dim3(pl.chunks, n, pl.gsplit)), dim3(256), 0, STREAM, (const bf16*)x0, c0, pitch0, (const bf16*)x1, c1, pitch1, hw, groups, pl.chunks, ws));
   return LADI_OK;
 }
 
 extern "C" int ladi_groupnorm_apply(const void* x0, int c0, int pitch0, const void* x1, int c1, int pitch1, int n, int hw, int groups,
                                     const float* ws, const float* gamma, const float* beta, float eps, int silu, const void* add,
                                     int add_pitch, void* out, int out_pitch, void* stream) {
-  if (int e = gn_check(x0, c0, pitch0, x1, c1, pitch1, groups)) return e;
-  LADI_CHECK(out_pitch % 8 == 0 && out_pitch >= c0 + c1, "groupnorm out pitch invalid");
-  const int chunks = gn_chunks(hw);
-  const int nv = (c0 + c1) / 8;
-  int ppb = (256 * 16) / nv;  // >= 16 vectors per thread, and few enough blocks that the per-block channel table amortises
-  const int target_blocks = (ladi_num_sms() * 3 + n - 1) / n;  // 3 resident blocks per SM (launch bounds): the whole grid is one wave
-  const int ppb2 = (hw + target_blocks - 1) / target_blocks;
-  if (ppb2 > ppb) ppb = ppb2;
-  if (ppb < 1) ppb = 1;
-  const int blocks = (hw + ppb - 1) / ppb;
+  ladi_gn_plan pl;
+  if (int e = gn_plan_apply(x0, c0, pitch0, x1, c1, pitch1, n, hw, groups, ws, gamma, beta, add, add_pitch, out, out_pitch, ladi_num_sms(), pl))
+    return e;
+  const int ppb = pl.px_per_block, blocks = pl.apply_blocks, chunks = pl.chunks;
   if (add != nullptr)
     LADI_CUDA(ladi_launch(gn_apply_kernel<true>, dim3(dim3(blocks, n)), dim3(256), 0, STREAM, (const bf16*)x0, c0, pitch0, (const bf16*)x1, c1, pitch1, hw, groups, chunks, ws,
                           gamma, beta, eps, silu, (const bf16*)add, add_pitch, (bf16*)out, out_pitch, ppb));
@@ -671,21 +717,44 @@ extern "C" int ladi_groupnorm_apply(const void* x0, int c0, int pitch0, const vo
   return LADI_OK;
 }
 
+// The LayerNorm launch's validation and shape: the smallest lane group T whose per-lane vector count VPL fits the register cache.
+static int ln_plan(const void* x, int x_pitch, int rows, int c, const float* gamma, const float* beta, const void* out, int out_pitch,
+                   ladi_ln_plan& pl) {
+  LADI_CHECK(c % 8 == 0 && c <= 2048, "layernorm: C %d must be a multiple of 8 and <= 2048", c);
+  LADI_CHECK(rows > 0, "layernorm: rows %d must be > 0", rows);
+  LADI_CHECK(x_pitch % 8 == 0 && x_pitch >= c, "layernorm x_pitch %d must be a multiple of 8 and >= C (%d)", x_pitch, c);
+  LADI_CHECK(out_pitch % 8 == 0 && out_pitch >= c, "layernorm out_pitch %d must be a multiple of 8 and >= C (%d)", out_pitch, c);
+  LADI_CHECK(x != nullptr && aligned16(x), "layernorm x %p must be non-null and 16-byte aligned", x);
+  LADI_CHECK(out != nullptr && aligned16(out), "layernorm out %p must be non-null and 16-byte aligned", out);
+  LADI_CHECK(gamma != nullptr && aligned16(gamma), "layernorm gamma %p must be non-null and 16-byte aligned", gamma);
+  LADI_CHECK(beta != nullptr && aligned16(beta), "layernorm beta %p must be non-null and 16-byte aligned", beta);
+  const int nv = c / 8;
+  pl.T = pl.vpl = 0;
+  for (int t = 4; t <= 32; t *= 2)
+    if (nv % t == 0 && nv / t <= 8) { pl.T = t; pl.vpl = nv / t; break; }
+  LADI_CHECK(pl.T != 0, "layernorm: unsupported width %d (need C/8 = T * v with T in {4,8,16,32}, v <= 8)", c);
+  pl.rows_per_block = 8 * (32 / pl.T);
+  pl.blocks = (rows + pl.rows_per_block - 1) / pl.rows_per_block;
+  return LADI_OK;
+}
+
+extern "C" int ladi_layernorm_plan(const void* x, int x_pitch, int rows, int c, const float* gamma, const float* beta, float eps,
+                                   const void* out, int out_pitch, int sms, ladi_ln_plan* plan) {
+  (void)eps; (void)sms;
+  LADI_CHECK(plan != nullptr, "plan output is null");
+  return ln_plan(x, x_pitch, rows, c, gamma, beta, out, out_pitch, *plan);
+}
+
 extern "C" int ladi_layernorm(const void* x, int x_pitch, int rows, int c, const float* gamma, const float* beta, float eps, void* out,
                               int out_pitch, void* stream) {
-  LADI_CHECK(c % 8 == 0 && c <= 2048 && x_pitch % 8 == 0 && out_pitch % 8 == 0, "layernorm: C must be a multiple of 8 and <= 2048");
-  const int nv = c / 8;
-  int T = 0, vpl = 0;
-  for (int t = 4; t <= 32; t *= 2)  // smallest lane group whose per-lane vector count fits the register cache
-    if (nv % t == 0 && nv / t <= 8) { T = t; vpl = nv / t; break; }
-  LADI_CHECK(T != 0, "layernorm: unsupported width %d (need C/8 = T * v with T in {4,8,16,32}, v <= 8)", c);
-  const int rows_per_block = 8 * (32 / T);
-  const int blocks = (rows + rows_per_block - 1) / rows_per_block;
+  ladi_ln_plan pl;
+  if (int e = ln_plan(x, x_pitch, rows, c, gamma, beta, out, out_pitch, pl)) return e;
+  const int T = pl.T, blocks = pl.blocks;
 #define LN_CASE(V) \
   case V: LADI_CUDA(ladi_launch(layernorm_kernel<V>, dim3(blocks), dim3(256), 0, STREAM, (const bf16*)x, x_pitch, rows, c, T, gamma, beta, eps, (bf16*)out, out_pitch)); break;
-  switch (vpl) {
+  switch (pl.vpl) {
     LN_CASE(1) LN_CASE(2) LN_CASE(3) LN_CASE(4) LN_CASE(5) LN_CASE(6) LN_CASE(7) LN_CASE(8)
-    default: LADI_CHECK(false, "layernorm: bad vectors per lane %d", vpl);
+    default: LADI_CHECK(false, "layernorm: bad vectors per lane %d", pl.vpl);
   }
 #undef LN_CASE
   return LADI_OK;

@@ -36,6 +36,15 @@ class ConvPlan(C.Structure):  # ladi_conv_plan: the path ladi_conv2d_bf16 takes 
         return (self.tiles_m + 1) // 2 * self.tiles_n if self.pair else self.tiles_m * self.tiles_n * self.splits
 
 
+class GroupNormPlan(C.Structure):  # ladi_gn_plan: the grids ladi_groupnorm_stats / ladi_groupnorm_apply launch
+    _fields_ = [(f, C.c_int) for f in ("chunks", "gsplit", "block_channels", "lanes_v", "k", "px_per_chunk", "px_per_block", "apply_blocks",
+                                        "dv", "dp", "slices")]
+
+
+class LayerNormPlan(C.Structure):  # ladi_ln_plan (ladi_layernorm_plan)
+    _fields_ = [(f, C.c_int) for f in ("T", "vpl", "rows_per_block", "blocks")]
+
+
 class AttnDesc(C.Structure):
     _fields_ = [
         ("batch", C.c_int), ("heads", C.c_int), ("nq", C.c_int), ("nkv", C.c_int),
@@ -77,7 +86,9 @@ SIGNATURES = {
     "ladi_groupnorm_chunks": ([_I], _I),
     "ladi_groupnorm_stats": ([_P, _I, _I, _P, _I, _I, _I, _I, _I, _P, _P], _I),
     "ladi_groupnorm_apply": ([_P, _I, _I, _P, _I, _I, _I, _I, _I, _P, _P, _P, _F, _I, _P, _I, _P, _I, _P], _I),
+    "ladi_groupnorm_plan": ([_P, _I, _I, _P, _I, _I, _I, _I, _I, _P, _P, _P, _F, _I, _P, _I, _P, _I, _I, C.POINTER(GroupNormPlan)], _I),
     "ladi_layernorm": ([_P, _I, _I, _I, _P, _P, _F, _P, _I, _P], _I),
+    "ladi_layernorm_plan": ([_P, _I, _I, _I, _P, _P, _F, _P, _I, _I, C.POINTER(LayerNormPlan)], _I),
     "ladi_softmax_rows": ([_P, _I, _I, _I, _F, _P, _I, _P], _I),
     "ladi_cls_attention": ([_P, _I, _P, _I, _I, _I, _I, _I, _F, _P, _I, _P], _I),
     "ladi_add_bf16": ([_P, _P, _P, _L, _P], _I),

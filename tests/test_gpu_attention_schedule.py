@@ -24,11 +24,22 @@ def _operand(R, B, n, width, pitch, bstride, std, col0=0, buf=None):
     return buf, vals
 
 
-def run_case(R, B, heads, nq, nkv, fused=False):
+def _late_max_keys(R, B, nkv, D, scale):
+    """Keys whose scores grow by 2 per 64-key tile along a direction every query shares: each tile holds a larger maximum than all
+    before it, so the online softmax rescales l and O on every tile."""
+    u = torch.sign(R.randn(D))
+    k = (R.randn(B, nkv, D) * 0.5 + (2.0 * (torch.arange(nkv, device=R.dev) // 64) / (scale * D))[None, :, None] * u).bfloat16()
+    return k, u
+
+
+def run_case(R, B, heads, nq, nkv, fused=False, D=64, late_max=False):
+    """D = 64: ladi_attention_bf16 with `heads` heads; D = 512 / 256: ladi_attention_d512_bf16 (heads must be 1, head_dim = D)."""
     from ladi_vton_b200 import lib
-    width = heads * 64
+    width = heads * D
+    scale = SCALE if D == 64 else D ** -0.5
     d = lib.AttnDesc()
-    d.batch, d.heads, d.nq, d.nkv, d.scale, d.variant = B, heads, nq, nkv, SCALE, 0
+    d.batch, d.heads, d.nq, d.nkv, d.scale, d.variant = B, heads, nq, nkv, scale, 0
+    d.head_dim = 0 if D == 64 else D
     if fused:  # one [B][n][3 * width + PAD] projection output: q, k, v are column slices of it
         assert nq == nkv
         pitch = 3 * width + PAD
@@ -45,6 +56,11 @@ def run_case(R, B, heads, nq, nkv, fused=False):
         pitch = width + PAD
         qb, q = _operand(R, B, nq, width, pitch, nq * pitch + GAP, 2 ** 0.5)
         kb, k = _operand(R, B, nkv, width, pitch, nkv * pitch + GAP, 2 ** 0.5)
+        if late_max:
+            k, u = _late_max_keys(R, B, nkv, D, scale)
+            q = (q.float() * 0.5 + u).bfloat16()
+            qb.as_strided((B, nq, width), (nq * pitch + GAP, pitch, 1)).copy_(q)
+            kb.as_strided((B, nkv, width), (nkv * pitch + GAP, pitch, 1)).copy_(k)
         vb, v = _operand(R, B, nkv, width, pitch, nkv * pitch + GAP, 1.0)
         d.q, d.q_pitch, d.q_batch_stride = qb.data_ptr(), pitch, nq * pitch + GAP
         d.k, d.k_pitch, d.k_batch_stride = kb.data_ptr(), pitch, nkv * pitch + GAP
@@ -56,7 +72,7 @@ def run_case(R, B, heads, nq, nkv, fused=False):
     for _ in range(2):
         o = torch.full(((B - 1) * obs + nq * op,), float("nan"), dtype=torch.bfloat16, device=R.dev)
         d.out = o.data_ptr()
-        lib.call("ladi_attention_bf16", C.byref(d), R.stream)
+        lib.call("ladi_attention_bf16" if D == 64 else "ladi_attention_d512_bf16", C.byref(d), R.stream)
         outs.append(o)
     torch.cuda.synchronize()
     del keep
@@ -68,7 +84,7 @@ def run_case(R, B, heads, nq, nkv, fused=False):
     assert _bitwise_equal(outs[0], outs[1]), "two runs differ bitwise"
     ov = out.as_strided((B, nq, width), (obs, op, 1))
     for b in range(B):
-        o64, sv = _attn_ref(q[b].double(), k[b].double(), v[b].double(), heads, 64, SCALE)
+        o64, sv = _attn_ref(q[b].double(), k[b].double(), v[b].double(), heads, D, scale)
         worst = float(ratio(ov[b], o64, attn_expect(o64, sv, nkv)).max())
         assert worst <= 1.0, f"image {b}: err/bound {worst:.3g}"
 
@@ -103,3 +119,40 @@ def test_persistent_ctas_run_several_items(cuda, B, heads, nq, nkv):
     # more (query tile, head, image) items than an H100 has SMs: CTAs carry the K / V ring, the Q double buffer and the warpgroups'
     # issue order from one item into the next
     run_case(Replay(cuda, B * heads + nq + nkv), B, heads, nq, nkv)
+
+
+# ================================================================================================================ head width 512 / 256
+# attention_kernel<D>: 128-row query tiles over two consumer warpgroups (64 rows each), 64-key tiles, a 10-stage ring of 64-column
+# chunks that one D = 512 tile fills exactly (8 K + 2 V chunks) and a D = 256 tile (4 + 2) wraps mid-tile, TMA zero-fill at nq / nkv.
+@pytest.mark.gpu
+@pytest.mark.parametrize("D", [512, 256])
+@pytest.mark.parametrize("nkv", [1, 63, 64, 65, 127, 64 * 101 + 5])
+def test_wide_key_counts(cuda, D, nkv):
+    run_case(Replay(cuda, 200 + nkv + D), 3, 1, 130, nkv, D=D)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("D", [512, 256])
+@pytest.mark.parametrize("nq", [1, 63, 64, 65, 127, 128, 129])
+def test_wide_query_tails(cuda, D, nq):
+    # nq = 1 .. 64: the second consumer warpgroup of the only query tile has no rows; 65: one
+    run_case(Replay(cuda, 300 + nq + D), 3, 1, nq, 150, D=D)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("D", [512, 256])
+def test_wide_fused_qkv_in_place(cuda, D):
+    run_case(Replay(cuda, 400 + D), 3, 1, 200, 200, fused=True, D=D)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("n_tiles", [1, 2, 5, 40])
+def test_d256_ring_wraps(cuda, n_tiles):
+    # 6 ring stages per key tile of 10: the ring wraps mid-tile from the second tile on
+    run_case(Replay(cuda, 500 + n_tiles), 3, 1, 160, 64 * n_tiles, D=256)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("D", [512, 256])
+def test_wide_late_maximum(cuda, D):
+    run_case(Replay(cuda, 600 + D), 3, 1, 200, 64 * 7 + 10, D=D, late_max=True)
