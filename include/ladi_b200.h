@@ -196,9 +196,20 @@ LADI_API int ladi_softmax_rows(const float* s, int rows, int cols, int s_pitch, 
 
 /* CLS-row attention of the inversion adapter's CLIP ViT-H encoder layer (16 heads, head_dim 80, 257 tokens): only token 0 of the
  * layer output is consumed (src/models/inversion_adapter.py:22-28), so only the CLS query is attended.
- * q0 [batch, heads*head_dim] bf16, kv [batch, tokens, >= 2*heads*head_dim] bf16 (K columns then V columns) -> out [batch, heads*head_dim]. */
+ * q0 [batch, heads*head_dim] bf16, kv [batch, tokens, >= 2*heads*head_dim] bf16 (K columns then V columns) -> out [batch, heads*head_dim].
+ * Placement rules (LADI_ERR_INVALID, naming the operand): kv 4-byte aligned with an even kv_pitch >= 2*heads*head_dim (K is read as
+ * bf16 pairs); q_pitch and out_pitch >= heads*head_dim; head_dim even.  Image b's K/V rows start at kv + b*tokens*kv_pitch.  The
+ * (head_dim + tokens) fp32 values of one block and its 16 bytes of static reduction slots must fit 48 KB: tokens <= 12204 at head_dim 80. */
 LADI_API int ladi_cls_attention(const void* q0, int q_pitch, const void* kv, int kv_pitch, int batch, int tokens, int heads, int head_dim,
                        float scale, void* out, int out_pitch, void* stream);
+/* The launch ladi_cls_attention runs for these arguments (ladi_sa_plan below): chunks = rows_per_block = 1 (one block per head and
+ * image, for the CLS row), its dynamic shared memory, never an opt-in.  `sms` is accepted like the other plan queries'; this plan does
+ * not depend on it.  The same validation code as the launch; dereferences no pointer, needs no device. */
+typedef struct ladi_sa_plan {
+  int chunks, rows_per_block, smem_bytes, smem_optin;
+} ladi_sa_plan;
+LADI_API int ladi_cls_attention_plan(const void* q0, int q_pitch, const void* kv, int kv_pitch, int batch, int tokens, int heads,
+                            int head_dim, float scale, const void* out, int out_pitch, int sms, ladi_sa_plan* plan);
 
 /* ---- pointwise glue ------------------------------------------------------------------------------------------------- */
 /* out = a + b (bf16, equal pitch-free dense [count]); VAE decoder `sample += int_feat` (vae.py:193). */
@@ -252,11 +263,23 @@ LADI_API int ladi_pose_heatmaps(const float* keypoints, int n_maps, int h, int w
  * Exact softmax attention for short sequences and any head width that is a multiple of 8 (<= 128), optional causal mask:
  * the CLIP text transformer driven by src/utils/encode_text_word_embedding.py:41-54 (77 causal tokens, 16 x 64) and the CLIP ViT-H
  * vision tower called at src/inference.py:269-273 (257 tokens, 16 x 80).  q/k/v/out: bf16 [batch, n, heads*head_dim] views with
- * row pitches and batch strides in elements (multiples of 8).  nkv <= 1024; causal needs nq == nkv. */
+ * row pitches and batch strides in elements (multiples of 8).  nkv <= 1024; causal needs nq == nkv.  Placement rules
+ * (LADI_ERR_INVALID, naming the operand): k and v 16-byte aligned (rows are read as 16-byte vectors), q and out 4-byte aligned (bf16
+ * pairs); every pitch >= heads*head_dim; for batch > 1 out_batch_stride >= nq*out_pitch (output images may not overlap; input images
+ * may).  K and V of one (image, head), the 8 warps' query rows and probabilities must fit 200 KB of shared memory: at head_dim 128,
+ * nkv <= 365; 1024 keys need head_dim <= 40. */
 LADI_API int ladi_attention_small(const void* q, const void* k, const void* v, void* out, int batch, int heads, int nq, int nkv,
                          int head_dim, int q_pitch, int k_pitch, int v_pitch, int out_pitch, long long q_batch_stride,
                          long long k_batch_stride, long long v_batch_stride, long long out_batch_stride, float scale, int causal,
                          void* stream);
+/* The launch ladi_attention_small runs for these arguments on a device with `sms` SMs (sms <= 0: the current device's): query-row
+ * chunks per (head, image) (blockIdx.x), query rows per 8-warp block (warp w takes rows w, w + 8, ... of its block), dynamic shared
+ * memory bytes, and whether they exceed the 48 KB a launch gets without raising the kernel's limit (smem_optin).  The same validation
+ * and policy code as the launch; it dereferences no pointer and needs no device. */
+LADI_API int ladi_attention_small_plan(const void* q, const void* k, const void* v, const void* out, int batch, int heads, int nq, int nkv,
+                              int head_dim, int q_pitch, int k_pitch, int v_pitch, int out_pitch, long long q_batch_stride,
+                              long long k_batch_stride, long long v_batch_stride, long long out_batch_stride, float scale,
+                              int causal, int sms, ladi_sa_plan* plan);
 /* out[row,:] = (src[row] >= 0 ? tok[src[row],:] : word_emb[-src[row]-1,:]) + pos[row % seq,:]  (bf16 tables, fp32 sum):
  * token_embedding + the '$' -> pseudo-word-embedding substitution + position_embedding of
  * src/utils/encode_text_word_embedding.py:27-38 (the index list `src` is built on the host from input_ids). */

@@ -176,33 +176,75 @@ __global__ void __launch_bounds__(128) vit_assemble_kernel(const bf16* __restric
 
 #define STREAM reinterpret_cast<cudaStream_t>(stream)
 
-extern "C" int ladi_attention_small(const void* q, const void* k, const void* v, void* out, int batch, int heads, int nq, int nkv,
-                                    int head_dim, int q_pitch, int k_pitch, int v_pitch, int out_pitch, long long q_batch_stride,
-                                    long long k_batch_stride, long long v_batch_stride, long long out_batch_stride, float scale,
-                                    int causal, void* stream) {
+static bool aligned_to(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
+// Everything ladi_attention_small decides, from its arguments and the SM count alone (no pointer is dereferenced, nothing touches a
+// device): validation, the dynamic shared memory of one (image, head) and the query-row split.  ladi_attention_small_plan reports it;
+// ladi_attention_small launches it.  The kernel reads K and V rows as 16-byte vectors and Q rows / writes O rows as bf16 pairs.
+static int sa_plan(const void* q, const void* k, const void* v, const void* out, int batch, int heads, int nq, int nkv, int head_dim,
+                   int q_pitch, int k_pitch, int v_pitch, int out_pitch, long long q_batch_stride, long long k_batch_stride,
+                   long long v_batch_stride, long long out_batch_stride, int causal, int sms, ladi_sa_plan& pl) {
   LADI_CHECK(q && k && v && out, "attention_small: null pointer");
   LADI_CHECK(batch > 0 && heads > 0 && nq > 0 && nkv > 0 && nkv <= 1024, "attention_small: bad extent (1 <= nkv <= 1024)");
   LADI_CHECK(head_dim >= 8 && head_dim <= 128 && head_dim % 8 == 0, "attention_small: head_dim must be a multiple of 8 in [8,128]");
   LADI_CHECK(q_pitch % 8 == 0 && k_pitch % 8 == 0 && v_pitch % 8 == 0 && out_pitch % 8 == 0 && q_batch_stride % 8 == 0 &&
                  k_batch_stride % 8 == 0 && v_batch_stride % 8 == 0 && out_batch_stride % 8 == 0,
              "attention_small: pitches and batch strides must be multiples of 8 elements");
+  LADI_CHECK(aligned_to(k, 16), "attention_small k %p must be 16-byte aligned", k);
+  LADI_CHECK(aligned_to(v, 16), "attention_small v %p must be 16-byte aligned", v);
+  LADI_CHECK(aligned_to(q, 4), "attention_small q %p must be 4-byte aligned", q);
+  LADI_CHECK(aligned_to(out, 4), "attention_small out %p must be 4-byte aligned", out);
+  const long long width = (long long)heads * head_dim;
+  LADI_CHECK(q_pitch >= width, "attention_small q_pitch %d is below heads*head_dim (%lld)", q_pitch, width);
+  LADI_CHECK(k_pitch >= width, "attention_small k_pitch %d is below heads*head_dim (%lld)", k_pitch, width);
+  LADI_CHECK(v_pitch >= width, "attention_small v_pitch %d is below heads*head_dim (%lld)", v_pitch, width);
+  LADI_CHECK(out_pitch >= width, "attention_small out_pitch %d is below heads*head_dim (%lld)", out_pitch, width);
+  LADI_CHECK(batch == 1 || out_batch_stride >= (long long)nq * out_pitch,
+             "attention_small out_batch_stride %lld is below nq*out_pitch (%lld): output images would overlap", out_batch_stride,
+             (long long)nq * out_pitch);
   LADI_CHECK(!causal || nq == nkv, "attention_small: the causal mask needs nq == nkv");
   const int hw = head_dim / 2, nkv_pad = (nkv + 31) & ~31;
   const size_t smem = ((size_t)nkv * (hw + 1) + (size_t)nkv * hw) * 4 + (size_t)SA_WARPS * nkv_pad * 4 + (size_t)SA_WARPS * head_dim * 4;
   LADI_CHECK(smem <= 200 * 1024, "attention_small: K/V of one head (%zu bytes) do not fit shared memory", smem);
-  static size_t configured = 0;
-  if (smem > configured) {
-    LADI_CUDA(cudaFuncSetAttribute(small_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = smem;
-  }
+  pl.smem_bytes = (int)smem;
+  pl.smem_optin = smem > 48 * 1024;
   // enough blocks to cover the GPU about twice, at least one query row per warp
-  int chunks = (2 * ladi_num_sms() + batch * heads - 1) / (batch * heads);
+  int chunks = (2 * sms + batch * heads - 1) / (batch * heads);
   int rpb = (nq + chunks - 1) / chunks;
   if (rpb < SA_WARPS) rpb = SA_WARPS;
-  chunks = (nq + rpb - 1) / rpb;
-  LADI_CUDA(ladi_launch(small_attention_kernel, dim3(chunks, heads, batch), dim3(SA_WARPS * 32), smem, STREAM, (const bf16*)q,
-                        (const bf16*)k, (const bf16*)v, (bf16*)out, nq, nkv, head_dim, q_pitch, k_pitch, v_pitch, out_pitch, q_batch_stride,
-                        k_batch_stride, v_batch_stride, out_batch_stride, scale * 1.4426950408889634f, causal, rpb));
+  pl.chunks = (nq + rpb - 1) / rpb;
+  pl.rows_per_block = rpb;
+  return LADI_OK;
+}
+
+extern "C" int ladi_attention_small_plan(const void* q, const void* k, const void* v, const void* out, int batch, int heads, int nq,
+                                         int nkv, int head_dim, int q_pitch, int k_pitch, int v_pitch, int out_pitch,
+                                         long long q_batch_stride, long long k_batch_stride, long long v_batch_stride,
+                                         long long out_batch_stride, float scale, int causal, int sms, ladi_sa_plan* plan) {
+  (void)scale;
+  LADI_CHECK(plan != nullptr, "plan output is null");
+  return sa_plan(q, k, v, out, batch, heads, nq, nkv, head_dim, q_pitch, k_pitch, v_pitch, out_pitch, q_batch_stride, k_batch_stride,
+                 v_batch_stride, out_batch_stride, causal, sms > 0 ? sms : ladi_num_sms(), *plan);
+}
+
+extern "C" int ladi_attention_small(const void* q, const void* k, const void* v, void* out, int batch, int heads, int nq, int nkv,
+                                    int head_dim, int q_pitch, int k_pitch, int v_pitch, int out_pitch, long long q_batch_stride,
+                                    long long k_batch_stride, long long v_batch_stride, long long out_batch_stride, float scale,
+                                    int causal, void* stream) {
+  ladi_sa_plan pl;
+  if (int e = sa_plan(q, k, v, out, batch, heads, nq, nkv, head_dim, q_pitch, k_pitch, v_pitch, out_pitch, q_batch_stride, k_batch_stride,
+                      v_batch_stride, out_batch_stride, causal, ladi_num_sms(), pl))
+    return e;
+  // the largest size this process has opted the kernel into; a smaller call needs no new attribute
+  static size_t configured = 0;
+  if ((size_t)pl.smem_bytes > configured) {
+    LADI_CUDA(cudaFuncSetAttribute(small_attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, pl.smem_bytes));
+    configured = pl.smem_bytes;
+  }
+  LADI_CUDA(ladi_launch(small_attention_kernel, dim3(pl.chunks, heads, batch), dim3(SA_WARPS * 32), (size_t)pl.smem_bytes, STREAM,
+                        (const bf16*)q, (const bf16*)k, (const bf16*)v, (bf16*)out, nq, nkv, head_dim, q_pitch, k_pitch, v_pitch, out_pitch,
+                        q_batch_stride, k_batch_stride, v_batch_stride, out_batch_stride, scale * 1.4426950408889634f, causal,
+                        pl.rows_per_block));
   return LADI_OK;
 }
 

@@ -338,6 +338,7 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const float* __restri
 // ---- CLS-row attention of the inversion adapter's CLIP encoder layer: only token 0 of the layer output is consumed
 // (src/models/inversion_adapter.py:26), so the query is the CLS row alone; one block per (head, image).
 //   q0 [B, heads*hd] (bias included, unscaled), kv [B, T, 2*heads*hd] (K then V), out [B, heads*hd]
+constexpr int CLS_WARPS = 4;  // 128 threads; their reduction slots are the kernel's only static shared memory
 __global__ void __launch_bounds__(128) cls_attention_kernel(const bf16* __restrict__ q0, int q_pitch, const bf16* __restrict__ kv,
                                                             int kv_pitch, int T, int heads, int hd, float scale, bf16* __restrict__ out,
                                                             int out_pitch) {
@@ -345,7 +346,7 @@ __global__ void __launch_bounds__(128) cls_attention_kernel(const bf16* __restri
   extern __shared__ float sm[];  // [hd] query, [T] probabilities
   float* sq = sm;
   float* sp = sm + hd;
-  __shared__ float red[4];
+  __shared__ float red[CLS_WARPS];
   const int h = blockIdx.x, b = blockIdx.y, t = threadIdx.x;
   const int C = heads * hd;
   for (int d = t; d < hd; d += 128) sq[d] = __bfloat162float(q0[(size_t)b * q_pitch + h * hd + d]) * scale;
@@ -766,14 +767,41 @@ extern "C" int ladi_softmax_rows(const float* s, int rows, int cols, int s_pitch
   return LADI_OK;
 }
 
+// ladi_cls_attention's validation and launch size, shared with ladi_cls_attention_plan: one block per (head, image) for the one CLS
+// row, dynamic shared memory for the query and the token probabilities.  The kernel reads K as bf16 pairs and everything else as
+// scalars.  Without an opt-in, static and dynamic shared memory together must fit 48 KB.
+static int cls_plan(const void* q0, int q_pitch, const void* kv, int kv_pitch, int batch, int tokens, int heads, int head_dim,
+                    const void* out, int out_pitch, ladi_sa_plan& pl) {
+  LADI_CHECK(q0 && kv && out && batch > 0 && tokens > 0 && heads > 0 && head_dim > 0 && head_dim % 2 == 0, "cls_attention: bad arguments");
+  LADI_CHECK(kv_pitch % 2 == 0, "cls_attention kv_pitch %d must be even", kv_pitch);
+  LADI_CHECK((reinterpret_cast<uintptr_t>(kv) & 3) == 0, "cls_attention kv %p must be 4-byte aligned", kv);
+  const long long width = (long long)heads * head_dim;
+  LADI_CHECK(kv_pitch >= 2 * width, "cls_attention kv_pitch %d is below 2*heads*head_dim (%lld)", kv_pitch, 2 * width);
+  LADI_CHECK(q_pitch >= width, "cls_attention q_pitch %d is below heads*head_dim (%lld)", q_pitch, width);
+  LADI_CHECK(out_pitch >= width, "cls_attention out_pitch %d is below heads*head_dim (%lld)", out_pitch, width);
+  const size_t smem = (size_t)(head_dim + tokens) * sizeof(float);
+  LADI_CHECK(smem + CLS_WARPS * sizeof(float) <= 48 * 1024, "cls_attention: too many tokens (%zu bytes of shared memory, %d tokens)",
+             smem + CLS_WARPS * sizeof(float), tokens);
+  pl.chunks = 1;
+  pl.rows_per_block = 1;
+  pl.smem_bytes = (int)smem;
+  pl.smem_optin = 0;
+  return LADI_OK;
+}
+
+extern "C" int ladi_cls_attention_plan(const void* q0, int q_pitch, const void* kv, int kv_pitch, int batch, int tokens, int heads,
+                                       int head_dim, float scale, const void* out, int out_pitch, int sms, ladi_sa_plan* plan) {
+  (void)scale; (void)sms;
+  LADI_CHECK(plan != nullptr, "plan output is null");
+  return cls_plan(q0, q_pitch, kv, kv_pitch, batch, tokens, heads, head_dim, out, out_pitch, *plan);
+}
+
 extern "C" int ladi_cls_attention(const void* q0, int q_pitch, const void* kv, int kv_pitch, int batch, int tokens, int heads, int head_dim,
                                   float scale, void* out, int out_pitch, void* stream) {
-  LADI_CHECK(q0 && kv && out && batch > 0 && tokens > 0 && heads > 0 && head_dim > 0 && head_dim % 2 == 0, "cls_attention: bad arguments");
-  LADI_CHECK(kv_pitch % 2 == 0 && (heads * head_dim) % 2 == 0, "cls_attention: pitches must be even");
-  const size_t smem = (size_t)(head_dim + tokens) * sizeof(float);
-  LADI_CHECK(smem <= 48 * 1024, "cls_attention: too many tokens");
-  LADI_CUDA(ladi_launch(cls_attention_kernel, dim3(heads, batch), dim3(128), smem, STREAM, (const bf16*)q0, q_pitch, (const bf16*)kv, kv_pitch, tokens,
-                        heads, head_dim, scale, (bf16*)out, out_pitch));
+  ladi_sa_plan pl;
+  if (int e = cls_plan(q0, q_pitch, kv, kv_pitch, batch, tokens, heads, head_dim, out, out_pitch, pl)) return e;
+  LADI_CUDA(ladi_launch(cls_attention_kernel, dim3(heads, batch), dim3(128), (size_t)pl.smem_bytes, STREAM, (const bf16*)q0, q_pitch,
+                        (const bf16*)kv, kv_pitch, tokens, heads, head_dim, scale, (bf16*)out, out_pitch));
   return LADI_OK;
 }
 

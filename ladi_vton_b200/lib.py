@@ -45,6 +45,10 @@ class LayerNormPlan(C.Structure):  # ladi_ln_plan (ladi_layernorm_plan)
     _fields_ = [(f, C.c_int) for f in ("T", "vpl", "rows_per_block", "blocks")]
 
 
+class SmallAttnPlan(C.Structure):  # ladi_sa_plan (ladi_attention_small_plan, ladi_cls_attention_plan)
+    _fields_ = [(f, C.c_int) for f in ("chunks", "rows_per_block", "smem_bytes", "smem_optin")]
+
+
 class AttnDesc(C.Structure):
     _fields_ = [
         ("batch", C.c_int), ("heads", C.c_int), ("nq", C.c_int), ("nkv", C.c_int),
@@ -91,6 +95,7 @@ SIGNATURES = {
     "ladi_layernorm_plan": ([_P, _I, _I, _I, _P, _P, _F, _P, _I, _I, C.POINTER(LayerNormPlan)], _I),
     "ladi_softmax_rows": ([_P, _I, _I, _I, _F, _P, _I, _P], _I),
     "ladi_cls_attention": ([_P, _I, _P, _I, _I, _I, _I, _I, _F, _P, _I, _P], _I),
+    "ladi_cls_attention_plan": ([_P, _I, _P, _I, _I, _I, _I, _I, _F, _P, _I, _I, C.POINTER(SmallAttnPlan)], _I),
     "ladi_add_bf16": ([_P, _P, _P, _L, _P], _I),
     "ladi_upsample2x_nhwc": ([_P, _I, _I, _I, _I, _P, _P], _I),
     "ladi_nchw_f32_to_nhwc_bf16": ([_P, _I, _I, _I, _I, _I, _F, _P, _P, _I, _I, _P], _I),
@@ -104,6 +109,8 @@ SIGNATURES = {
     "ladi_image_out_u8": ([_P, _I, _I, _I, _I, _I, _P, _P], _I),
     "ladi_pose_heatmaps": ([_P, _I, _I, _I, _F, _P, _P], _I),
     "ladi_attention_small": ([_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _L, _L, _L, _L, _F, _I, _P], _I),
+    "ladi_attention_small_plan": ([_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _L, _L, _L, _L, _F, _I, _I,
+                                   C.POINTER(SmallAttnPlan)], _I),
     "ladi_clip_embed": ([_P, _P, _P, _P, _P, _I, _I, _I, _I, _P], _I),
     "ladi_patchify": ([_P, _P, _I, _I, _I, _I, _I, _I, _P], _I),
     "ladi_vit_assemble": ([_P, _I, _P, _P, _P, _I, _I, _I, _P], _I),

@@ -276,11 +276,26 @@ def softmax_rows(s, scale, out=None):
 
 def cls_attention(q0, kv, heads, head_dim, scale):
     """q0 [B, heads*hd] bf16 (CLS query), kv [B, T, 2*heads*hd] bf16 (K | V) -> [B, heads*hd] bf16."""
+    args, out = _cls_attention_args(q0, kv, heads, head_dim, scale)
+    lib.call("ladi_cls_attention", *args, _stream())
+    return out
+
+
+def cls_attention_plan(q0, kv, heads, head_dim, scale):
+    """The launch (lib.SmallAttnPlan) cls_attention(q0, kv, heads, head_dim, scale) runs; launches nothing.  Invalid -> RuntimeError."""
+    args, _ = _cls_attention_args(q0, kv, heads, head_dim, scale)
+    plan = lib.SmallAttnPlan()
+    L = lib.load()
+    if L.ladi_cls_attention_plan(*args, 0, C.byref(plan)) != 0:
+        raise RuntimeError(f"ladi_cls_attention_plan failed: {L.ladi_last_error().decode()}")
+    return plan
+
+
+def _cls_attention_args(q0, kv, heads, head_dim, scale):
     B, T = kv.shape[0], kv.shape[1]
     assert q0.dtype == torch.bfloat16 and kv.dtype == torch.bfloat16 and kv.stride(2) == 1 and q0.stride(1) == 1
     out = torch.empty((B, heads * head_dim), dtype=torch.bfloat16, device=q0.device)
-    lib.call("ladi_cls_attention", _ptr(q0), q0.stride(0), _ptr(kv), kv.stride(1), B, T, heads, head_dim, scale, _ptr(out), out.stride(0), _stream())
-    return out
+    return (_ptr(q0), q0.stride(0), _ptr(kv), kv.stride(1), B, T, heads, head_dim, scale, _ptr(out), out.stride(0)), out
 
 
 def add(a, b, out=None):
@@ -387,16 +402,32 @@ def pose_heatmaps(keypoints, h, w, sigma=9.0):
 def attention_small(q, k, v, heads, scale, causal=False):
     """q [B, Nq, heads*hd], k/v [B, Nkv, heads*hd] bf16 views (last dim contiguous) -> [B, Nq, heads*hd] bf16.  Exact softmax,
     fp32 scores; any head width that is a multiple of 8 (the CLIP ViT-H heads are 80 wide), Nkv <= 1024, optional causal mask."""
+    args, out = _attention_small_args(q, k, v, heads, scale, causal)
+    B, nq, nkv, hd = args[4], args[6], args[7], args[8]
+    _call("ladi_attention_small", 4.0 * B * heads * nq * nkv * hd, *args, _stream(), tag=f"B={B} heads={heads} nq={nq} nkv={nkv} hd={hd}")
+    return out
+
+
+def attention_small_plan(q, k, v, heads, scale, causal=False, sms=0):
+    """The launch (lib.SmallAttnPlan: query-row chunks per head and image, rows per block, shared memory, opt-in) attention_small(q, k, v,
+    heads, scale, causal) runs on a device with `sms` SMs (0: this one's); launches nothing.  Invalid -> RuntimeError."""
+    args, _ = _attention_small_args(q, k, v, heads, scale, causal)
+    plan = lib.SmallAttnPlan()
+    L = lib.load()
+    if L.ladi_attention_small_plan(*args, sms, C.byref(plan)) != 0:
+        raise RuntimeError(f"ladi_attention_small_plan failed: {L.ladi_last_error().decode()}")
+    return plan
+
+
+def _attention_small_args(q, k, v, heads, scale, causal):
+    """-> (the arguments of ladi_attention_small without the stream, the output tensor they write)."""
     B, nq, C = q.shape
-    nkv = k.shape[1]
     hd = C // heads
     for t in (q, k, v):
         assert t.dtype == torch.bfloat16 and t.stride(2) == 1
     out = torch.empty((B, nq, C), dtype=torch.bfloat16, device=q.device)
-    _call("ladi_attention_small", 4.0 * B * heads * nq * nkv * hd, _ptr(q), _ptr(k), _ptr(v), _ptr(out), B, heads, nq, nkv, hd,
-          q.stride(1), k.stride(1), v.stride(1), out.stride(1), q.stride(0), k.stride(0), v.stride(0), out.stride(0), float(scale),
-          1 if causal else 0, _stream(), tag=f"B={B} heads={heads} nq={nq} nkv={nkv} hd={hd}")
-    return out
+    return (_ptr(q), _ptr(k), _ptr(v), _ptr(out), B, heads, nq, k.shape[1], hd, q.stride(1), k.stride(1), v.stride(1), out.stride(1),
+            q.stride(0), k.stride(0), v.stride(0), out.stride(0), float(scale), 1 if causal else 0), out
 
 
 def clip_embed(src, tok, word_emb, pos, seq):

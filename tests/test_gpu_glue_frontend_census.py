@@ -1040,8 +1040,7 @@ def replay_tps_grid(R, f):
 
 
 def replay_attention_small(R, f):
-    from ladi_vton_b200 import lib
-    B, heads, nq, nkv, hd, causal, scale = (f[k] for k in ("B", "heads", "nq", "nkv", "hd", "causal", "scale"))
+    B, heads, nq, nkv, hd = (f[k] for k in ("B", "heads", "nq", "nkv", "hd"))
     Cw = heads * hd
     bufs = {}
     for nm, n_, std in (("q", nq, 2 ** 0.5), ("k", nkv, 2 ** 0.5), ("v", nkv, 1.0)):
@@ -1049,6 +1048,16 @@ def replay_attention_small(R, f):
         t = torch.full(((B - 1) * bs + n_ * p,), NAN, dtype=torch.bfloat16, device=R.dev)
         t.as_strided((B, n_, Cw), (bs, p, 1)).copy_(R.randn(B, n_, Cw, std=std).bfloat16())
         bufs[nm] = t
+    return check_attention_small(R, f, bufs)
+
+
+def check_attention_small(R, f, bufs):
+    """Run the descriptor f twice on the inputs bufs["q" / "k" / "v"] (bf16 tensors whose storage offset is the operand's address; they
+    may be views into one buffer) into a NaN-poisoned output with a tail, then check the layout, determinism and the float64 bound of
+    every query row of every image."""
+    from ladi_vton_b200 import lib
+    B, heads, nq, nkv, hd, causal, scale = (f[k] for k in ("B", "heads", "nq", "nkv", "hd", "causal", "scale"))
+    Cw = heads * hd
     op, obs = f["op"], f["obs"]
     size = (B - 1) * obs + nq * op
 

@@ -520,20 +520,32 @@ def replay_attn(R, f):
 
 
 def replay_cls(R, f):
-    from ladi_vton_b200 import lib
     B, T, heads, hd = f["batch"], f["tokens"], f["heads"], f["hd"]
     Cw = heads * hd
     q0 = R.poisoned(B, f["qp"], R.randn(B, Cw, std=2 ** 0.5))
     kv = R.poisoned(B * T, f["kvp"], torch.cat([R.randn(B * T, Cw, std=2 ** 0.5), R.randn(B * T, Cw)], dim=1))
-    scale = hd ** -0.5  # csrc/engine.cu adapter_forward
+    return check_cls(R, f, q0, kv, hd ** -0.5)  # the scale of csrc/engine.cu adapter_forward
+
+
+CLS_TAIL = 3  # NaN rows after the output that no call may write
+
+
+def check_cls(R, f, q0, kv, scale):
+    """Run the descriptor f twice on q0 [B, qp] and kv [B * T, kvp] (NaN in their pitch gaps) into a NaN-poisoned output with CLS_TAIL
+    extra rows, then check the layout, determinism and the float64 bound."""
+    from ladi_vton_b200 import lib
+    B, T, heads, hd = f["batch"], f["tokens"], f["heads"], f["hd"]
+    Cw = heads * hd
     outs = []
     for _ in range(2):
-        o = R.poisoned(B, f["op"])
+        o = R.poisoned(B + CLS_TAIL, f["op"])
         lib.call("ladi_cls_attention", C.c_void_p(q0.data_ptr()), f["qp"], C.c_void_p(kv.data_ptr()), f["kvp"], B, T, heads, hd, scale,
                  C.c_void_p(o.data_ptr()), f["op"], R.stream)
         outs.append(o)
     torch.cuda.synchronize()
-    errs = _layout(outs[0], Cw, "output")
+    errs = _layout(outs[0][:B], Cw, "output")
+    if not bool(torch.isnan(outs[0][B:].float()).all()):
+        errs.append("output: wrote past the last image")
     if not _bitwise_equal(outs[0], outs[1]):
         errs.append("two runs differ bitwise")
     if errs:
