@@ -332,14 +332,16 @@ LADI_API int ladi_nhwc_f32_to_nchw_clamp(const float* x, int n, int c, int h, in
  * (ky*kw + kx)*c + ch, zeros in columns [kh*kw*c, k_pad); then one ladi_conv2d_bf16 GEMM (ksize 1).  x_is_f32_nchw = 0: x NHWC bf16 of
  * channel pitch `pitch` (c % 8 == 0), shift = scale = NULL.  x_is_f32_nchw = 1: x NCHW fp32 pixels, each in-image pixel becomes
  * (x - shift[ch]) / scale[ch] BEFORE the zero padding (LPIPS ScalingLayer ahead of AlexNet's padded 11x11 conv, lpips/pretrained_networks;
- * the FID Inception's (x - 128) / 128).  ladi_patchify is the special case patch = stride, no padding. */
+ * the FID Inception's (x - 128) / 128).  ladi_patchify is the special case patch = stride, no padding.  Placement rules (LADI_ERR_INVALID,
+ * naming the operand): NHWC form x and out 16-byte aligned; pixel form x, shift and scale 4-byte aligned, out 2-byte aligned. */
 LADI_API int ladi_im2col_bf16(const void* x, int x_is_f32_nchw, int n, int c, int h, int w, int pitch, int kh, int kw, int sh, int sw, int ph,
                               int pw, const float* shift, const float* scale, void* out, int k_pad, void* stream);
 /* torch max_pool2d / avg_pool2d (ceil_mode=False) on NHWC bf16 (c, pitches and c_off multiples of 8): window k, stride s, padding p,
  * output [n, (h+2p-k)/s+1, (w+2p-k)/s+1] written to channels [c_off, c_off+c) of `out` (pitch out_pitch) -- an Inception branch writes
  * straight into its Mixed_* concatenation.  Modes: MAX (padding never wins), AVG (count_include_pad=True, torchvision InceptionA/C/E),
  * AVG_EXCLUDE_PAD (count_include_pad=False, the FID blocks of pytorch-fid / torch-fidelity), GLOBAL_AVG_F32 (adaptive_avg_pool2d(x, 1):
- * `out` is fp32 [n, out_pitch], k / s / p ignored -- the Inception pool3 features). */
+ * `out` is fp32 [n, out_pitch], k / s / p ignored -- the Inception pool3 features).  Placement rules (LADI_ERR_INVALID, naming the
+ * operand): window modes x and out 16-byte aligned; GLOBAL_AVG_F32 x 2-byte and out 4-byte aligned. */
 #define LADI_POOL_MAX 0
 #define LADI_POOL_AVG 1
 #define LADI_POOL_AVG_EXCLUDE_PAD 2
@@ -349,16 +351,17 @@ LADI_API int ladi_pool2d_bf16(const void* x, int n, int h, int w, int c, int x_p
 /* One LPIPS layer (lpips.LPIPS.forward, version 0.1; torchmetrics LearnedPerceptualImagePatchSimilarity): feature pairs fa, fb NHWC bf16
  * [n, h, w, pitch]; per pixel n_a = a / (sqrt(sum_c a^2) + 1e-10), n_b likewise, d = sum_c lin[c] * (n_a - n_b)^2 (the 1x1 C -> 1 `lin`
  * conv, no bias, fp32 weights); acc[b] += mean over the h*w pixels of d.  Called once per AlexNet tap, acc (fp32 [n]) ends as the LPIPS
- * distance of each pair. */
+ * distance of each pair.  Placement rules (LADI_ERR_INVALID, naming the operand): fa, fb 2-byte aligned, lin and acc 4-byte aligned. */
 LADI_API int ladi_lpips_layer(const void* fa, const void* fb, int n, int h, int w, int c, int pitch, const float* lin, float* acc, void* stream);
 /* SSIM of torchmetrics StructuralSimilarityIndexMeasure(data_range=1.0) per image: x, y NCHW fp32; gaussian window 11 wide, sigma 1.5
  * (separable), C1 = 0.01^2, C2 = 0.03^2; the mean over channels and the (h-10) x (w-10) positions whose window lies inside the image
  * (torchmetrics reflect-pads by 5 and crops 5, which is the same).  fp32 throughout; ws: fp32 [n * ladi_ssim_partials(h, w)] of tile sums;
- * out fp32 [n].  h, w >= 11. */
+ * out fp32 [n].  h, w >= 11, n <= 65535 (one grid.z slice per image).  x, y, ws and out 4-byte aligned (LADI_ERR_INVALID otherwise). */
 LADI_API int ladi_ssim_partials(int h, int w);
 LADI_API int ladi_ssim_f32(const float* x, const float* y, int n, int c, int h, int w, float* ws, float* out, void* stream);
 /* The Inception Score input of torchmetrics InceptionScore(normalize=True): (x * 255).byte() then torch-fidelity's TF1-style bilinear resize
- * (source coordinate o * in/out, no half-pixel offset, upper neighbour clamped): x NCHW fp32 in [0, 1] -> out NCHW fp32 [n, c, oh, ow]. */
+ * (source coordinate o * in/out, no half-pixel offset, upper neighbour clamped): x NCHW fp32 in [0, 1] -> out NCHW fp32 [n, c, oh, ow].
+ * x and out 4-byte aligned (LADI_ERR_INVALID otherwise). */
 LADI_API int ladi_resize_tf1_u8(const float* x, int n, int c, int h, int w, int oh, int ow, float* out, void* stream);
 
 /* ================================================================================================================================

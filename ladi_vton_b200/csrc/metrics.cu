@@ -265,6 +265,8 @@ __global__ void __launch_bounds__(256) resize_tf1_kernel(const float* __restrict
 
 }  // namespace
 
+static bool aligned_to(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
 #define STREAM reinterpret_cast<cudaStream_t>(stream)
 
 extern "C" int ladi_im2col_bf16(const void* x, int x_is_f32_nchw, int n, int c, int h, int w, int pitch, int kh, int kw, int sh, int sw, int ph,
@@ -276,11 +278,17 @@ extern "C" int ladi_im2col_bf16(const void* x, int x_is_f32_nchw, int n, int c, 
   const long long rows = (long long)n * oh * ow;
   if (x_is_f32_nchw) {
     LADI_CHECK(shift && scale, "im2col: the pixel form needs shift and scale");
+    LADI_CHECK(aligned_to(x, 4), "im2col: x %p must be 4-byte aligned (fp32 pixels)", x);
+    LADI_CHECK(aligned_to(shift, 4), "im2col: shift %p must be 4-byte aligned", shift);
+    LADI_CHECK(aligned_to(scale, 4), "im2col: scale %p must be 4-byte aligned", scale);
+    LADI_CHECK(aligned_to(out, 2), "im2col: out %p must be 2-byte aligned", out);
     LADI_CUDA(ladi_launch(im2col_pixels_kernel, dim3(grid_for(rows * k_pad)), dim3(256), 0, STREAM, (const float*)x, c, h, w, kh, kw, sh, sw, ph,
                           pw, oh, ow, rows, shift, scale, (bf16*)out, k_pad));
   } else {
     LADI_CHECK(!shift && !scale, "im2col: shift / scale apply to the fp32 pixel form only");
     LADI_CHECK(c % 8 == 0 && pitch % 8 == 0 && pitch >= c, "im2col: C and pitch must be multiples of 8");
+    LADI_CHECK(aligned_to(x, 16), "im2col: x %p must be 16-byte aligned", x);
+    LADI_CHECK(aligned_to(out, 16), "im2col: out %p must be 16-byte aligned", out);
     LADI_CUDA(ladi_launch(im2col_nhwc_kernel, dim3(grid_for(rows * (k_pad / 8))), dim3(256), 0, STREAM, (const bf16*)x, h, w, c, pitch, kh, kw, sh,
                           sw, ph, pw, oh, ow, rows, (bf16*)out, k_pad));
   }
@@ -293,6 +301,8 @@ extern "C" int ladi_pool2d_bf16(const void* x, int n, int h, int w, int c, int x
   LADI_CHECK(c % 8 == 0 && x_pitch % 8 == 0 && x_pitch >= c, "pool2d: C and pitch must be multiples of 8");
   if (mode == LADI_POOL_GLOBAL_AVG_F32) {
     LADI_CHECK(out_pitch >= c_off + c, "pool2d: channel window outside the output pitch");
+    LADI_CHECK(aligned_to(x, 2), "pool2d: x %p must be 2-byte aligned", x);
+    LADI_CHECK(aligned_to(out, 4), "pool2d: out %p must be 4-byte aligned (fp32 features)", out);
     LADI_CUDA(ladi_launch(global_avg_kernel, dim3(grid_for((long long)n * c)), dim3(256), 0, STREAM, (const bf16*)x, n, h * w, c, x_pitch,
                           (float*)out + c_off, out_pitch));
     return LADI_OK;
@@ -300,6 +310,8 @@ extern "C" int ladi_pool2d_bf16(const void* x, int n, int h, int w, int c, int x
   LADI_CHECK(mode == LADI_POOL_MAX || mode == LADI_POOL_AVG || mode == LADI_POOL_AVG_EXCLUDE_PAD, "pool2d: unknown mode %d", mode);
   LADI_CHECK(k > 0 && s > 0 && p >= 0 && 2 * p <= k && h + 2 * p >= k && w + 2 * p >= k, "pool2d: bad window (k %d, s %d, p %d)", k, s, p);
   LADI_CHECK(out_pitch % 8 == 0 && c_off % 8 == 0 && out_pitch >= c_off + c, "pool2d: output pitch / channel offset must be multiples of 8");
+  LADI_CHECK(aligned_to(x, 16), "pool2d: x %p must be 16-byte aligned", x);
+  LADI_CHECK(aligned_to(out, 16), "pool2d: out %p must be 16-byte aligned", out);
   const int oh = (h + 2 * p - k) / s + 1, ow = (w + 2 * p - k) / s + 1;
   const long long pixels = (long long)n * oh * ow;
   LADI_CUDA(ladi_launch(pool2d_kernel, dim3(grid_for(pixels * (c / 8))), dim3(256), 0, STREAM, (const bf16*)x, h, w, c, x_pitch, k, s, p, mode, oh,
@@ -309,6 +321,10 @@ extern "C" int ladi_pool2d_bf16(const void* x, int n, int h, int w, int c, int x
 
 extern "C" int ladi_lpips_layer(const void* fa, const void* fb, int n, int h, int w, int c, int pitch, const float* lin, float* acc, void* stream) {
   LADI_CHECK(fa && fb && lin && acc && n > 0 && h > 0 && w > 0 && c > 0 && pitch >= c, "lpips_layer: bad extent");
+  LADI_CHECK(aligned_to(fa, 2), "lpips_layer: fa %p must be 2-byte aligned", fa);
+  LADI_CHECK(aligned_to(fb, 2), "lpips_layer: fb %p must be 2-byte aligned", fb);
+  LADI_CHECK(aligned_to(lin, 4), "lpips_layer: lin %p must be 4-byte aligned", lin);
+  LADI_CHECK(aligned_to(acc, 4), "lpips_layer: acc %p must be 4-byte aligned", acc);
   LADI_CUDA(ladi_launch(lpips_layer_kernel, dim3(n), dim3(LPIPS_WARPS * 32), 0, STREAM, (const bf16*)fa, (const bf16*)fb, h * w, c, pitch, lin, acc));
   return LADI_OK;
 }
@@ -321,6 +337,11 @@ extern "C" int ladi_ssim_partials(int h, int w) {
 extern "C" int ladi_ssim_f32(const float* x, const float* y, int n, int c, int h, int w, float* ws, float* out, void* stream) {
   LADI_CHECK(x && y && ws && out && n > 0 && c > 0, "ssim: bad arguments");
   LADI_CHECK(h >= SSIM_K && w >= SSIM_K, "ssim: images must be at least 11 x 11 (got %d x %d)", h, w);
+  LADI_CHECK(n <= 65535, "ssim: n %d exceeds 65535 images per call (one grid.z slice per image)", n);
+  LADI_CHECK(aligned_to(x, 4), "ssim: x %p must be 4-byte aligned", x);
+  LADI_CHECK(aligned_to(y, 4), "ssim: y %p must be 4-byte aligned", y);
+  LADI_CHECK(aligned_to(ws, 4), "ssim: ws %p must be 4-byte aligned", ws);
+  LADI_CHECK(aligned_to(out, 4), "ssim: out %p must be 4-byte aligned", out);
   const dim3 grid((w - SSIM_K + 1 + SSIM_T - 1) / SSIM_T, (h - SSIM_K + 1 + SSIM_T - 1) / SSIM_T, n);
   LADI_CUDA(ladi_launch(ssim_tile_kernel, grid, dim3(SSIM_T, SSIM_T), 0, STREAM, x, y, c, h, w, ws));
   const float inv = (float)(1.0 / ((double)c * (h - SSIM_K + 1) * (w - SSIM_K + 1)));
@@ -330,6 +351,8 @@ extern "C" int ladi_ssim_f32(const float* x, const float* y, int n, int c, int h
 
 extern "C" int ladi_resize_tf1_u8(const float* x, int n, int c, int h, int w, int oh, int ow, float* out, void* stream) {
   LADI_CHECK(x && out && n > 0 && c > 0 && h > 0 && w > 0 && oh > 0 && ow > 0, "resize_tf1: bad extent");
+  LADI_CHECK(aligned_to(x, 4), "resize_tf1: x %p must be 4-byte aligned", x);
+  LADI_CHECK(aligned_to(out, 4), "resize_tf1: out %p must be 4-byte aligned", out);
   LADI_CUDA(ladi_launch(resize_tf1_kernel, dim3(grid_for((long long)n * c * oh * ow)), dim3(256), 0, STREAM, x, h, w, oh, ow, (long long)n * c, out));
   return LADI_OK;
 }

@@ -24,7 +24,7 @@ import math
 import numpy as np
 import torch
 
-from . import ops
+from . import lib, ops
 from .weights import pad64
 
 INCEPTION_BN_EPS = 1e-3
@@ -297,7 +297,8 @@ class FIDInceptionV3(_Net):
     def __call__(self, pixels):
         """pixels: NCHW fp32 [n, 3, 299, 299] with values in [0, 255] -> pool3 features fp32 [n, 2048] (device)."""
         self._check_ready()
-        assert pixels.dtype == torch.float32 and pixels.dim() == 4 and pixels.shape[1] == 3 and pixels.device.type == "cuda"
+        # CPU tensors only while the ABI calls are recorded instead of launched (tests/test_gpu_metrics_census.py)
+        assert pixels.dtype == torch.float32 and pixels.dim() == 4 and pixels.shape[1] == 3 and (pixels.device.type == "cuda" or lib.RECORD is not None)
         L = self.layers
         x = L["Conv2d_1a_3x3"](pixels.contiguous(), shift=self.shift, scale=self.scale)
         x = L["Conv2d_2b_3x3"](L["Conv2d_2a_3x3"](x))

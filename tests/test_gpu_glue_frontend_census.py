@@ -218,9 +218,9 @@ def _val(a):
     return getattr(a, "value", a)
 
 
-def describe(name, args):
-    """-> (kind, OrderedDict of fields) of one recorded call; raises KeyError for an entry point without a SCHEMA row."""
-    kind, spec = SCHEMA[name]
+def describe(name, args, schema=None):
+    """-> (kind, OrderedDict of fields) of one recorded call; raises KeyError for an entry point without a row in `schema` (default SCHEMA)."""
+    kind, spec = (SCHEMA if schema is None else schema)[name]
     names = spec.split()
     assert len(names) == len(args), f"{name}: {len(args)} arguments recorded, SCHEMA names {len(names)}"
     f = OrderedDict()
