@@ -211,21 +211,27 @@ typedef struct ladi_sa_plan {
 LADI_API int ladi_cls_attention_plan(const void* q0, int q_pitch, const void* kv, int kv_pitch, int batch, int tokens, int heads,
                             int head_dim, float scale, const void* out, int out_pitch, int sms, ladi_sa_plan* plan);
 
-/* ---- pointwise glue ------------------------------------------------------------------------------------------------- */
-/* out = a + b (bf16, equal pitch-free dense [count]); VAE decoder `sample += int_feat` (vae.py:193). */
+/* ---- pointwise glue ------------------------------------------------------------------------------------------------- *
+ * Every entry point below returns LADI_ERR_INVALID, naming the operand, for a null operand, an extent <= 0 or a placement its rules
+ * exclude; nothing is launched then. */
+/* out = a + b (bf16, equal pitch-free dense [count]); VAE decoder `sample += int_feat` (vae.py:193).  count a multiple of 8; a, b and
+ * out 16-byte aligned (8-element vectors). */
 LADI_API int ladi_add_bf16(const void* a, const void* b, void* out, int64_t count, void* stream);
-/* nearest 2x upsample NHWC (diffusers Upsample2D F.interpolate(scale_factor=2, mode="nearest")). */
+/* nearest 2x upsample NHWC (diffusers Upsample2D F.interpolate(scale_factor=2, mode="nearest")).  Dense, c a multiple of 8; x and out
+ * 16-byte aligned. */
 LADI_API int ladi_upsample2x_nhwc(const void* x, int n, int h, int w, int c, void* out, void* stream);
 /* NCHW fp32 [n,c,h*f,w*f] -> NHWC bf16 [n,h,w,pitch] channels [c_off, c_off+c): nearest sampling every f-th pixel
  * (F.interpolate default mode, tryon_pipe.py:434-436), times `scale`, optionally gated by (gate[n,0,..] < 0.5) -- the
- * `masked_image = image * (mask < 0.5)` of diffusers prepare_mask_and_masked_image (call-site tryon_pipe.py:630). */
+ * `masked_image = image * (mask < 0.5)` of diffusers prepare_mask_and_masked_image (call-site tryon_pipe.py:630).  f >= 1,
+ * c_off >= 0 and out_pitch >= c_off + c. */
 LADI_API int ladi_nchw_f32_to_nhwc_bf16(const float* x, int n, int c, int h, int w, int f, float scale, const float* gate, void* out,
                                int out_pitch, int c_off, void* stream);
-/* NHWC (bf16 or fp32) -> NCHW fp32, channels [c_off, c_off+c) of an NHWC tensor of given pitch. */
+/* NHWC (bf16 or fp32) -> NCHW fp32, channels [c_off, c_off+c) of an NHWC tensor of given pitch: c_off >= 0, x_pitch >= c_off + c. */
 LADI_API int ladi_nhwc_to_nchw_f32(const void* x, int x_is_fp32, int n, int c, int h, int w, int x_pitch, int c_off, float* out,
                           void* stream);
 /* DiagonalGaussianDistribution.sample * scaling_factor (vae.py:330-348; tryon_pipe.py:647,462):
- * moments NHWC fp32 [n,h,w,2*cz] -> latents NCHW fp32 [n,cz,h,w] = (mean + exp(0.5*clamp(logvar,-30,20))*noise) * scale. */
+ * moments NHWC fp32 [n,h,w,2*cz] -> latents NCHW fp32 [n,cz,h,w] = (mean + exp(0.5*clamp(logvar,-30,20))*noise) * scale; m_pitch >= 2*cz.
+ * A NaN logvar stays NaN through the clamp, as torch.clamp keeps it. */
 LADI_API int ladi_posterior_sample(const float* moments, int m_pitch, const float* noise_nchw, int n, int cz, int h, int w, float scale,
                           float* out_nchw, void* stream);
 /* mask (1 - m) rows for EMASC mask_features (src/utils/data_utils.py:9-14): mask NCHW fp32 [n,1,H,W] nearest-resized by
@@ -238,17 +244,20 @@ LADI_API int ladi_bilinear_down8(const float* x, int n, int c, int H, int W, flo
  * in place; unet_in NHWC bf16 [cfg?2B:B, h, w, in_pitch] channels 0..3 rewritten for both halves.  coef = device table
  * [steps][8] = {1/sqrt(a_t), sqrt(1-a_t), sqrt(a_prev), sqrt(1-a_prev-sigma_t^2), sigma_t, 0, 0, 0}, indexed by *step_ptr, which is
  * then incremented by the last block when advance != 0.  noise: NCHW fp32 [B,4,h,w] variance noise of the eta > 0 (stochastic)
- * DDIM update, x_prev += sigma_t * noise; NULL for eta = 0. */
+ * DDIM update, x_prev += sigma_t * noise; NULL for eta = 0.  eps_pitch >= 4 and in_pitch >= 4; advance != 0 needs step_ptr (the
+ * counter it advances; with step_ptr NULL the call reads coefficient row 0 and cannot advance). */
 LADI_API int ladi_ddim_cfg_step(const float* eps, int eps_pitch, float* latents, void* unet_in, int in_pitch, int B, int h, int w,
                        int cfg, float guidance, const float* coef, int* step_ptr, int advance, const float* noise, void* stream);
 /* diffusers prepare_mask_and_masked_image, tensor branch (called at tryon_pipe.py:630), without host synchronisation: range checks
  * image in [-1,1] / mask in [0,1] recorded in flags[0] / flags[1] (device int32[2], OR-ed; the pipeline reads them once, with the result)
  * and the IN-PLACE binarisation of the caller's mask at 0.5.  image fp32 [n_image], mask fp32 [n_mask], both dense. */
 LADI_API int ladi_check_binarise(const float* image, long long n_image, float* mask, long long n_mask, int* flags, void* stream);
-/* (x/2+0.5).clamp(0,1) NHWC bf16/fp32 [n,h,w,pitch] (first 3 channels) -> NHWC fp32 [n,h,w,3] (tryon_pipe.py:356-358). */
+/* (x/2+0.5).clamp(0,1) NHWC bf16/fp32 [n,h,w,pitch] (first 3 channels) -> NHWC fp32 [n,h,w,3] (tryon_pipe.py:356-358); x_pitch >= 3.
+ * NaN stays NaN, as torch.clamp keeps it. */
 LADI_API int ladi_image_out(const void* x, int x_is_fp32, int n, int h, int w, int x_pitch, float* out, void* stream);
 /* The same clamp followed by numpy_to_pil's (x * 255).round().astype(uint8) (DiffusionPipeline.numpy_to_pil, called at
- * tryon_pipe.py:760; round-half-to-even like numpy): NHWC uint8 [n,h,w,3], so output_type="pil" moves a quarter of the bytes to the host. */
+ * tryon_pipe.py:760; round-half-to-even like numpy): NHWC uint8 [n,h,w,3], so output_type="pil" moves a quarter of the bytes to the host.
+ * x_pitch >= 3.  NaN gives 0 (numpy's NaN -> uint8 cast has no defined value). */
 LADI_API int ladi_image_out_u8(const void* x, int x_is_fp32, int n, int h, int w, int x_pitch, unsigned char* out, void* stream);
 /* Sinusoidal timestep embedding of the UNet (diffusers get_timestep_embedding, flip_sin_to_cos, the input of time_embedding.linear_1; SURVEY App. A.2)
  * for n timesteps (device fp32 [n]), written as a (hi, lo) pair of bf16 column blocks: out bf16 [n, 2*k_pad], hi at columns [0, channels),
@@ -282,13 +291,15 @@ LADI_API int ladi_attention_small_plan(const void* q, const void* k, const void*
                               int causal, int sms, ladi_sa_plan* plan);
 /* out[row,:] = (src[row] >= 0 ? tok[src[row],:] : word_emb[-src[row]-1,:]) + pos[row % seq,:]  (bf16 tables, fp32 sum):
  * token_embedding + the '$' -> pseudo-word-embedding substitution + position_embedding of
- * src/utils/encode_text_word_embedding.py:27-38 (the index list `src` is built on the host from input_ids). */
+ * src/utils/encode_text_word_embedding.py:27-38 (the index list `src` is built on the host from input_ids).  c and out_pitch
+ * multiples of 8; tok, pos, out and word_emb (NULL when no row is negative) 16-byte aligned. */
 LADI_API int ladi_clip_embed(const int* src, const void* tok, const void* word_emb, const void* pos, void* out, int rows, int seq, int c,
                     int out_pitch, void* stream);
 /* pixels NCHW fp32 [n,ch,h,w] -> bf16 rows [n*(h/patch)*(w/patch), k_pad], column (c*patch+ky)*patch+kx, zero padding columns:
  * the im2col of CLIPVisionEmbeddings.patch_embedding (14x14 stride-14 convolution, no bias), followed by one ladi_conv2d_bf16 GEMM. */
 LADI_API int ladi_patchify(const float* pixels, void* out, int n, int ch, int h, int w, int patch, int k_pad, void* stream);
-/* x[b,0,:] = cls + pos[0,:]; x[b,1+i,:] = patch[b*n_patches+i,:] + pos[1+i,:]  (CLIPVisionEmbeddings.forward), all bf16. */
+/* x[b,0,:] = cls + pos[0,:]; x[b,1+i,:] = patch[b*n_patches+i,:] + pos[1+i,:]  (CLIPVisionEmbeddings.forward), all bf16.  c and
+ * patch_pitch multiples of 8, patch_pitch >= c; patch, cls, pos and out 16-byte aligned; n <= 65535 (one grid.y slice per image). */
 LADI_API int ladi_vit_assemble(const void* patch, int patch_pitch, const void* cls, const void* pos, void* out, int n, int n_patches, int c,
                       void* stream);
 
@@ -304,25 +315,31 @@ LADI_API int ladi_clip_preprocess(const float* x, int n, int c, int h, int w, in
 /* NHWC bf16 [n,h,w,c] -> [n,h/2,w/2,4c], channel (sy*2+sx)*c+ch <- pixel (2y+sy, 2x+sx): the 4x4 stride-2 pad-1 convolutions of
  * FeatureExtraction / FeatureRegression (ConvNet_TPS.py:31-38,93-97) become 3x3 stride-1 pad-1 ladi_conv2d_bf16 calls. */
 LADI_API int ladi_space_to_depth2(const void* x, int n, int h, int w, int c, int x_pitch, void* out, int out_pitch, void* stream);
-/* in place x[row,c] = x[row,c]*scale[c] + shift[c]: eval-mode BatchNorm2d that follows a ReLU (ConvNet_TPS.py:33,39,41). */
+/* in place x[row,c] = x[row,c]*scale[c] + shift[c]: eval-mode BatchNorm2d that follows a ReLU (ConvNet_TPS.py:33,39,41).  c and pitch
+ * multiples of 8; x, scale and shift 16-byte aligned (scale / shift are read as float4). */
 LADI_API int ladi_channel_affine(void* x, long long rows, int c, int pitch, const float* scale, const float* shift, void* stream);
-/* FeatureL2Norm (ConvNet_TPS.py:58-66), in place over the channel dimension of NHWC bf16 rows. */
+/* FeatureL2Norm (ConvNet_TPS.py:58-66), in place over the channel dimension of NHWC bf16 rows.  c and pitch multiples of 8; x 16-byte
+ * aligned. */
 LADI_API int ladi_l2norm_channels(void* x, long long rows, int c, int pitch, void* stream);
-/* FeatureCorrelation (ConvNet_TPS.py:69-81): out NHWC bf16 [n,h,w,h*w], out[b,yB,xB,xA*h+yA] = <B[b,yB,xB,:], A[b,yA,xA,:]>. */
+/* FeatureCorrelation (ConvNet_TPS.py:69-81): out NHWC bf16 [n,h,w,h*w], out[b,yB,xB,xA*h+yA] = <B[b,yB,xB,:], A[b,yA,xA,:]>.  Dense
+ * inputs, c a multiple of 8; feat_a and feat_b 16-byte aligned; out_pitch >= h*w. */
 LADI_API int ladi_feature_correlation(const void* feat_a, const void* feat_b, int n, int h, int w, int c, void* out, int out_pitch, void* stream);
 /* points = tanh(theta) (ConvNet_TPS.py:122); grid = target_coordinate_repr @ (inverse_kernel @ [points; 0]) (TPSGridGen.forward,
  * :183-193).  theta fp32 [n, >= 2*n_ctrl]; inverse_kernel [(n_ctrl+3)^2]; target_coordinate_repr [n_points, n_ctrl+3];
- * points fp32 [n, n_ctrl, 2]; grid fp32 [n, n_points, 2]. */
+ * points fp32 [n, n_ctrl, 2]; grid fp32 [n, n_points, 2].  1 <= n_ctrl <= 64, theta_pitch >= 2*n_ctrl, n <= 65535 (one grid.y slice
+ * per image). */
 LADI_API int ladi_tps_grid(const float* theta, int theta_pitch, const float* inverse_kernel, const float* target_coordinate_repr, int n, int n_ctrl,
                   int n_points, float* points, float* grid, void* stream);
 /* inference.py:252-257: antialiased-bilinear resize of low_grid fp32 [n,gh,gw,2] to (h,w) fused with F.grid_sample(cloth, grid,
  * bilinear, padding_mode='border', align_corners=False); cloth NCHW fp32 [n,c,h,w] -> channels [c_off,c_off+c) of NHWC bf16 out. */
 LADI_API int ladi_warp_grid_sample(const float* low_grid, int gh, int gw, const float* cloth, int n, int c, int h, int w, void* out, int out_pitch,
                           int c_off, void* stream);
-/* nn.MaxPool2d(2) / nn.Upsample(scale_factor=2, bilinear, align_corners=True) on NHWC bf16 (unet_parts.py:31-34,47). */
+/* nn.MaxPool2d(2) / nn.Upsample(scale_factor=2, bilinear, align_corners=True) on NHWC bf16 (unet_parts.py:31-34,47).  Dense, c a
+ * multiple of 8; x and out 16-byte aligned.  The max pool returns NaN for a window holding a NaN, as nn.MaxPool2d does. */
 LADI_API int ladi_maxpool2_nhwc(const void* x, int n, int h, int w, int c, void* out, void* stream);
 LADI_API int ladi_upsample2x_bilinear_ac(const void* x, int n, int h, int w, int c, void* out, void* stream);
-/* NHWC fp32 [n,h,w,pitch] (first c channels) -> NCHW fp32 clamped to [lo,hi] (inference.py:262 warped_cloth.clamp(-1,1)). */
+/* NHWC fp32 [n,h,w,pitch] (first c channels) -> NCHW fp32 clamped to [lo,hi] (inference.py:262 warped_cloth.clamp(-1,1)); NaN stays
+ * NaN, as torch.clamp keeps it. */
 LADI_API int ladi_nhwc_f32_to_nchw_clamp(const float* x, int n, int c, int h, int w, int x_pitch, float lo, float hi, float* out, void* stream);
 
 /* ---- image-quality metrics (csrc/metrics.cu; the engine form of src/utils/val_metrics.py:105-225, which runs clean-fid's FID / KID

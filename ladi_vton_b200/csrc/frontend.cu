@@ -252,6 +252,10 @@ extern "C" int ladi_clip_embed(const int* src, const void* tok, const void* word
                                int c, int out_pitch, void* stream) {
   LADI_CHECK(src && tok && pos && out && rows > 0 && seq > 0, "clip_embed: bad arguments");
   LADI_CHECK(c % 8 == 0 && out_pitch % 8 == 0 && out_pitch >= c, "clip_embed: width must be a multiple of 8");
+  LADI_CHECK(aligned_to(tok, 16), "clip_embed: tok %p must be 16-byte aligned", tok);
+  LADI_CHECK(aligned_to(word_emb, 16), "clip_embed: word_emb %p must be 16-byte aligned", word_emb);
+  LADI_CHECK(aligned_to(pos, 16), "clip_embed: pos %p must be 16-byte aligned", pos);
+  LADI_CHECK(aligned_to(out, 16), "clip_embed: out %p must be 16-byte aligned", out);
   LADI_CUDA(ladi_launch(clip_embed_kernel, dim3(rows), dim3(128), 0, STREAM, src, (const bf16*)tok, (const bf16*)word_emb, (const bf16*)pos,
                         (bf16*)out, seq, c, out_pitch));
   return LADI_OK;
@@ -272,6 +276,12 @@ extern "C" int ladi_vit_assemble(const void* patch, int patch_pitch, const void*
                                  int c, void* stream) {
   LADI_CHECK(patch && cls && pos && out && n > 0 && n_patches > 0, "vit_assemble: bad arguments");
   LADI_CHECK(c % 8 == 0 && patch_pitch % 8 == 0, "vit_assemble: width must be a multiple of 8");
+  LADI_CHECK(patch_pitch >= c, "vit_assemble: patch_pitch %d is below c (%d)", patch_pitch, c);
+  LADI_CHECK(n <= 65535, "vit_assemble: n %d exceeds 65535 images per call (one grid.y slice per image)", n);
+  LADI_CHECK(aligned_to(patch, 16), "vit_assemble: patch %p must be 16-byte aligned", patch);
+  LADI_CHECK(aligned_to(cls, 16), "vit_assemble: cls %p must be 16-byte aligned", cls);
+  LADI_CHECK(aligned_to(pos, 16), "vit_assemble: pos %p must be 16-byte aligned", pos);
+  LADI_CHECK(aligned_to(out, 16), "vit_assemble: out %p must be 16-byte aligned", out);
   LADI_CUDA(ladi_launch(vit_assemble_kernel, dim3(n_patches + 1, n), dim3(128), 0, STREAM, (const bf16*)patch, patch_pitch, (const bf16*)cls,
                         (const bf16*)pos, (bf16*)out, n_patches, c));
   return LADI_OK;

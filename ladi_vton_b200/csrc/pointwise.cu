@@ -455,7 +455,7 @@ __global__ void posterior_kernel(const float* __restrict__ mom, int m_pitch, con
     const int64_t b = r / cz;
     const float* m = mom + (b * hw + px) * m_pitch;
     const float mean = m[ch];
-    const float logvar = fminf(fmaxf(m[cz + ch], -30.f), 20.f);
+    const float logvar = ptx::clamp_keep_nan(m[cz + ch], -30.f, 20.f);  // torch.clamp(logvar, -30, 20): a NaN logvar stays NaN
     out[i] = (mean + expf(0.5f * logvar) * noise[i]) * scale;
   }
 }
@@ -558,12 +558,13 @@ __global__ void image_out_kernel(const void* __restrict__ x, int is_f32, int64_t
     const int ch = (int)(i % 3);
     const float v = is_f32 ? reinterpret_cast<const float*>(x)[px * x_pitch + ch]
                            : __bfloat162float(reinterpret_cast<const bf16*>(x)[px * x_pitch + ch]);
-    out[i] = fminf(fmaxf(v * 0.5f + 0.5f, 0.f), 1.f);
+    out[i] = ptx::clamp_keep_nan(v * 0.5f + 0.5f, 0.f, 1.f);  // (image / 2 + 0.5).clamp(0, 1) keeps NaN
   }
 }
 
 // numpy_to_pil of the reference pipeline base class (called at tryon_pipe.py:760): (x * 255).round().astype(uint8) of the clamped
 // image, on the device -- the D2H copy shrinks 4x and the host only wraps the bytes in PIL images.  rintf = round-half-to-even = numpy.
+// NaN becomes 0 here (numpy's NaN -> uint8 cast is undefined; fmaxf picks the 0).
 __global__ void image_out_u8_kernel(const void* __restrict__ x, int is_f32, int64_t npx, int x_pitch, uint8_t* __restrict__ out) {
   ptx::pdl_wait();
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < npx * 3; i += (int64_t)gridDim.x * blockDim.x) {
@@ -806,43 +807,56 @@ extern "C" int ladi_cls_attention(const void* q0, int q_pitch, const void* kv, i
 }
 
 extern "C" int ladi_add_bf16(const void* a, const void* b, void* out, int64_t count, void* stream) {
-  LADI_CHECK(count % 8 == 0, "add: count must be a multiple of 8");
+  LADI_CHECK(a && b && out && count >= 0 && count % 8 == 0, "add: null operand, or count not a multiple of 8");
+  LADI_CHECK(aligned16(a), "add: a %p must be 16-byte aligned", a);
+  LADI_CHECK(aligned16(b), "add: b %p must be 16-byte aligned", b);
+  LADI_CHECK(aligned16(out), "add: out %p must be 16-byte aligned", out);
   LADI_CUDA(ladi_launch(add_kernel, dim3(grid_for(count / 8)), dim3(256), 0, STREAM, (const uint4*)a, (const uint4*)b, (uint4*)out, count / 8));
   return LADI_OK;
 }
 
 extern "C" int ladi_upsample2x_nhwc(const void* x, int n, int h, int w, int c, void* out, void* stream) {
-  LADI_CHECK(c % 8 == 0, "upsample: C must be a multiple of 8");
+  LADI_CHECK(x && out && n > 0 && h > 0 && w > 0 && c > 0 && c % 8 == 0, "upsample: bad extent (C must be a multiple of 8)");
+  LADI_CHECK(aligned16(x), "upsample: x %p must be 16-byte aligned", x);
+  LADI_CHECK(aligned16(out), "upsample: out %p must be 16-byte aligned", out);
   LADI_CUDA(ladi_launch(upsample2x_kernel, dim3(grid_for((int64_t)n * 4 * h * w * (c / 8))), dim3(256), 0, STREAM, (const uint4*)x, n, h, w, c / 8, (uint4*)out));
   return LADI_OK;
 }
 
 extern "C" int ladi_nchw_f32_to_nhwc_bf16(const float* x, int n, int c, int h, int w, int f, float scale, const float* gate, void* out,
                                           int out_pitch, int c_off, void* stream) {
-  LADI_CHECK(f >= 1, "nchw_to_nhwc: bad sampling factor");
+  LADI_CHECK(x && out && n > 0 && c > 0 && h > 0 && w > 0 && f >= 1, "nchw_to_nhwc: bad extent or sampling factor");
+  LADI_CHECK(c_off >= 0 && out_pitch >= c_off + c, "nchw_to_nhwc: channel window [%d, %d) outside the output pitch %d", c_off, c_off + c,
+             out_pitch);
   LADI_CUDA(ladi_launch(nchw_to_nhwc_kernel, dim3(grid_for((int64_t)n * c * h * w)), dim3(256), 0, STREAM, x, n, c, h, w, f, scale, gate, (bf16*)out, out_pitch, c_off));
   return LADI_OK;
 }
 
 extern "C" int ladi_nhwc_to_nchw_f32(const void* x, int x_is_fp32, int n, int c, int h, int w, int x_pitch, int c_off, float* out,
                                      void* stream) {
+  LADI_CHECK(x && out && n > 0 && c > 0 && h > 0 && w > 0, "nhwc_to_nchw: bad extent");
+  LADI_CHECK(c_off >= 0 && x_pitch >= c_off + c, "nhwc_to_nchw: channel window [%d, %d) outside the input pitch %d", c_off, c_off + c, x_pitch);
   LADI_CUDA(ladi_launch(nhwc_to_nchw_kernel, dim3(grid_for((int64_t)n * c * h * w)), dim3(256), 0, STREAM, x, x_is_fp32, n, c, h * w, x_pitch, c_off, out));
   return LADI_OK;
 }
 
 extern "C" int ladi_posterior_sample(const float* moments, int m_pitch, const float* noise_nchw, int n, int cz, int h, int w, float scale,
                                      float* out_nchw, void* stream) {
+  LADI_CHECK(moments && noise_nchw && out_nchw && n > 0 && cz > 0 && h > 0 && w > 0, "posterior_sample: bad extent");
+  LADI_CHECK(m_pitch >= 2 * cz, "posterior_sample: m_pitch %d is below 2*cz (%d): mean and logvar are read from one row", m_pitch, 2 * cz);
   LADI_CUDA(ladi_launch(posterior_kernel, dim3(grid_for((int64_t)n * cz * h * w)), dim3(256), 0, STREAM, moments, m_pitch, noise_nchw, n, cz, h * w, scale, out_nchw));
   return LADI_OK;
 }
 
 extern "C" int ladi_inv_mask_rows(const float* mask, int n, int H, int W, int f, float* out, void* stream) {
+  LADI_CHECK(mask && out && n > 0 && H > 0 && W > 0, "inv_mask: null operand or bad extent");
   LADI_CHECK(f >= 1 && H % f == 0 && W % f == 0, "inv_mask: factor must divide H and W");
   LADI_CUDA(ladi_launch(inv_mask_kernel, dim3(grid_for((int64_t)n * (H / f) * (W / f))), dim3(256), 0, STREAM, mask, n, H, W, f, out));
   return LADI_OK;
 }
 
 extern "C" int ladi_bilinear_down8(const float* x, int n, int c, int H, int W, float* out, void* stream) {
+  LADI_CHECK(x && out && n > 0 && c > 0 && H > 0 && W > 0, "bilinear_down8: null operand or bad extent");
   LADI_CHECK(H % 8 == 0 && W % 8 == 0, "bilinear_down8: H, W must be multiples of 8");
   LADI_CUDA(ladi_launch(bilinear8_kernel, dim3(grid_for((int64_t)n * c * (H / 8) * (W / 8))), dim3(256), 0, STREAM, x, n * c, H, W, out));
   return LADI_OK;
@@ -850,7 +864,10 @@ extern "C" int ladi_bilinear_down8(const float* x, int n, int c, int H, int W, f
 
 extern "C" int ladi_ddim_cfg_step(const float* eps, int eps_pitch, float* latents, void* unet_in, int in_pitch, int B, int h, int w,
                                   int cfg, float guidance, const float* coef, int* step_ptr, int advance, const float* noise, void* stream) {
-  LADI_CHECK(eps && latents && unet_in && coef, "ddim: null operand");
+  LADI_CHECK(eps && latents && unet_in && coef && B > 0 && h > 0 && w > 0, "ddim: null operand or bad extent");
+  LADI_CHECK(eps_pitch >= 4, "ddim: eps_pitch %d is below the 4 latent channels", eps_pitch);
+  LADI_CHECK(in_pitch >= 4, "ddim: in_pitch %d is below the 4 latent channels", in_pitch);
+  LADI_CHECK(!advance || step_ptr, "ddim: advance needs step_ptr (the step counter it advances)");
   LADI_CUDA(ladi_launch(ddim_cfg_kernel, dim3(grid_for((int64_t)B * 4 * h * w)), dim3(256), 0, STREAM, eps, eps_pitch, latents, (bf16*)unet_in, in_pitch, B, h * w, cfg,
                                                                          guidance, coef, step_ptr, advance, noise));
   return LADI_OK;
@@ -877,6 +894,7 @@ extern "C" int ladi_pose_heatmaps(const float* keypoints, int n_maps, int h, int
 }
 
 extern "C" int ladi_image_out(const void* x, int x_is_fp32, int n, int h, int w, int x_pitch, float* out, void* stream) {
+  LADI_CHECK(x && out && n > 0 && h > 0 && w > 0 && x_pitch >= 3, "image_out: bad extent");
   LADI_CUDA(ladi_launch(image_out_kernel, dim3(grid_for((int64_t)n * h * w * 3)), dim3(256), 0, STREAM, x, x_is_fp32, (int64_t)n * h * w, x_pitch, out));
   return LADI_OK;
 }

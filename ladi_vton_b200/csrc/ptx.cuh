@@ -209,5 +209,7 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
 }
 __device__ __forceinline__ float bf16_lo(uint32_t u) { return __uint_as_float(u << 16); }
 __device__ __forceinline__ float bf16_hi(uint32_t u) { return __uint_as_float(u & 0xFFFF0000u); }
+// torch.clamp(v, lo, hi): NaN stays NaN (fminf / fmaxf alone return the other operand)
+__device__ __forceinline__ float clamp_keep_nan(float v, float lo, float hi) { return v != v ? v : fminf(fmaxf(v, lo), hi); }
 
 }  // namespace ptx

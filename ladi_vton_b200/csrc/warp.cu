@@ -263,8 +263,10 @@ __global__ void __launch_bounds__(256) warp_sample_kernel(const float* __restric
   }
 }
 
+// NaN-propagating, as nn.MaxPool2d: a NaN anywhere in the window gives NaN (fmaxf would return the other operand)
 __device__ __forceinline__ uint32_t max2(uint32_t a, uint32_t b) {
-  return ptx::pack_bf16(fmaxf(ptx::bf16_lo(a), ptx::bf16_lo(b)), fmaxf(ptx::bf16_hi(a), ptx::bf16_hi(b)));
+  const __nv_bfloat162 r = __hmax2_nan(*reinterpret_cast<const __nv_bfloat162*>(&a), *reinterpret_cast<const __nv_bfloat162*>(&b));
+  return *reinterpret_cast<const uint32_t*>(&r);
 }
 // nn.MaxPool2d(2) on NHWC bf16 (unet_parts.py:31-34)
 __global__ void __launch_bounds__(256) maxpool2_kernel(const bf16* __restrict__ x, int n, int h, int w, int c, bf16* __restrict__ out) {
@@ -330,7 +332,7 @@ __global__ void __launch_bounds__(256) nhwc_to_nchw_clamp_kernel(const float* __
     const long long px = i % hw, r = i / hw;
     const int ch = (int)(r % c);
     const long long b = r / c;
-    out[i] = fminf(fmaxf(x[(b * hw + px) * pitch + ch], lo), hi);
+    out[i] = ptx::clamp_keep_nan(x[(b * hw + px) * pitch + ch], lo, hi);  // torch.clamp keeps NaN
   }
 }
 
@@ -341,6 +343,8 @@ inline int grid_for(long long total) {
 }
 
 }  // namespace
+
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 #define STREAM reinterpret_cast<cudaStream_t>(stream)
 
@@ -372,12 +376,16 @@ extern "C" int ladi_space_to_depth2(const void* x, int n, int h, int w, int c, i
 
 extern "C" int ladi_channel_affine(void* x, long long rows, int c, int pitch, const float* scale, const float* shift, void* stream) {
   LADI_CHECK(x && scale && shift && rows > 0 && c % 8 == 0 && pitch % 8 == 0 && pitch >= c, "channel_affine: C and pitch must be multiples of 8");
+  LADI_CHECK(aligned16(x), "channel_affine: x %p must be 16-byte aligned", x);
+  LADI_CHECK(aligned16(scale), "channel_affine: scale %p must be 16-byte aligned (read as float4)", scale);
+  LADI_CHECK(aligned16(shift), "channel_affine: shift %p must be 16-byte aligned (read as float4)", shift);
   LADI_CUDA(ladi_launch(channel_affine_kernel, dim3(grid_for(rows * (c / 8))), dim3(256), 0, STREAM, (bf16*)x, rows, c, pitch, scale, shift));
   return LADI_OK;
 }
 
 extern "C" int ladi_l2norm_channels(void* x, long long rows, int c, int pitch, void* stream) {
   LADI_CHECK(x && rows > 0 && c % 8 == 0 && pitch % 8 == 0 && pitch >= c, "l2norm: C and pitch must be multiples of 8");
+  LADI_CHECK(aligned16(x), "l2norm: x %p must be 16-byte aligned", x);
   LADI_CUDA(ladi_launch(l2norm_kernel, dim3((unsigned)((rows + 7) / 8)), dim3(256), 0, STREAM, (bf16*)x, rows, c, pitch));
   return LADI_OK;
 }
@@ -386,6 +394,8 @@ extern "C" int ladi_feature_correlation(const void* feat_a, const void* feat_b, 
                                         void* stream) {
   LADI_CHECK(feat_a && feat_b && out && n > 0 && h > 0 && w > 0 && c % 8 == 0, "correlation: C must be a multiple of 8");
   LADI_CHECK(out_pitch >= h * w, "correlation: output pitch below h*w");
+  LADI_CHECK(aligned16(feat_a), "correlation: fa %p must be 16-byte aligned", feat_a);
+  LADI_CHECK(aligned16(feat_b), "correlation: fb %p must be 16-byte aligned", feat_b);
   LADI_CUDA(ladi_launch(correlation_kernel, dim3(grid_for((long long)n * h * w * h * w)), dim3(256), 0, STREAM, (const bf16*)feat_a,
                         (const bf16*)feat_b, n, h, w, c, (bf16*)out, out_pitch));
   return LADI_OK;
@@ -395,6 +405,7 @@ extern "C" int ladi_tps_grid(const float* theta, int theta_pitch, const float* i
                              int n_ctrl, int n_points, float* points, float* grid, void* stream) {
   LADI_CHECK(theta && inverse_kernel && target_coordinate_repr && points && grid && n > 0 && n_points > 0, "tps_grid: bad arguments");
   LADI_CHECK(n_ctrl > 0 && n_ctrl <= TPS_MAXN && theta_pitch >= 2 * n_ctrl, "tps_grid: 1..64 control points");
+  LADI_CHECK(n <= 65535, "tps_grid: n %d exceeds 65535 images per call (one grid.y slice per image)", n);
   LADI_CUDA(ladi_launch(tps_grid_kernel, dim3((n_points + 255) / 256, n), dim3(256), 0, STREAM, theta, theta_pitch, inverse_kernel,
                         target_coordinate_repr, n_ctrl, n_points, points, grid));
   return LADI_OK;
@@ -412,6 +423,8 @@ extern "C" int ladi_warp_grid_sample(const float* low_grid, int gh, int gw, cons
 
 extern "C" int ladi_maxpool2_nhwc(const void* x, int n, int h, int w, int c, void* out, void* stream) {
   LADI_CHECK(x && out && n > 0 && h % 2 == 0 && w % 2 == 0 && c % 8 == 0, "maxpool2: even H, W and C %% 8 == 0");
+  LADI_CHECK(aligned16(x), "maxpool2: x %p must be 16-byte aligned", x);
+  LADI_CHECK(aligned16(out), "maxpool2: out %p must be 16-byte aligned", out);
   LADI_CUDA(ladi_launch(maxpool2_kernel, dim3(grid_for((long long)n * (h / 2) * (w / 2) * (c / 8))), dim3(256), 0, STREAM, (const bf16*)x, n, h, w,
                         c, (bf16*)out));
   return LADI_OK;
@@ -419,6 +432,8 @@ extern "C" int ladi_maxpool2_nhwc(const void* x, int n, int h, int w, int c, voi
 
 extern "C" int ladi_upsample2x_bilinear_ac(const void* x, int n, int h, int w, int c, void* out, void* stream) {
   LADI_CHECK(x && out && n > 0 && h > 0 && w > 0 && c % 8 == 0, "upsample2x_bilinear_ac: C %% 8 == 0");
+  LADI_CHECK(aligned16(x), "upsample2x_bilinear_ac: x %p must be 16-byte aligned", x);
+  LADI_CHECK(aligned16(out), "upsample2x_bilinear_ac: out %p must be 16-byte aligned", out);
   LADI_CUDA(ladi_launch(upsample2x_ac_kernel, dim3(grid_for((long long)n * 4 * h * w * (c / 8))), dim3(256), 0, STREAM, (const bf16*)x, n, h, w, c,
                         (bf16*)out));
   return LADI_OK;

@@ -439,11 +439,15 @@ def _tail_nan(flat, n, what):
 
 
 def _exact(y, r, what):
-    """bit-exact comparison (NaN allowed where the reference has it) -> ([error], (0 or inf, where))."""
+    """bit-exact comparison (NaN allowed where the reference has it, whatever its payload) -> ([error], (0 or inf, where))."""
     if _same(y.contiguous(), r.contiguous()):
         return [], (0.0, "bit-exact")
     it = {torch.bfloat16: torch.int16, torch.float32: torch.int32}.get(y.dtype)
-    bad = (y.view(it) != r.view(it)) if it is not None else (y != r)
+    bad = (y.contiguous().view(it) != r.contiguous().view(it)) if it is not None else (y != r)
+    if it is not None:
+        bad &= ~(torch.isnan(y) & torch.isnan(r))
+        if not bool(bad.any()):
+            return [], (0.0, "bit-exact, NaN where the reference has NaN")
     loc = [int(v) for v in bad.nonzero()[0]]
     msg = f"{what}: {int(bad.sum())} elements differ; first at index {loc}: got {y[tuple(loc)].item()}, ref {r[tuple(loc)].item()}"
     return [msg], (float("inf"), msg)
@@ -493,12 +497,14 @@ def _binary_mask(R, *shape):
     return torch.where(R.rand(*shape) < 0.02, torch.full_like(m, 0.5), m)
 
 
-def replay_nchw_to_nhwc(R, f):
+def replay_nchw_to_nhwc(R, f, gate_nan=False):
     from ladi_vton_b200 import lib
     n, c, h, w, fct, op, c_off = f["n"], f["c"], f["h"], f["w"], f["f"], f["op"], f["c_off"]
     H, W = h * fct, w * fct
     x = _image(R, n, c, H, W) if f["scale"] == 1.0 else R.randn(n, c, H, W)  # scale != 1: the latents the VAE decoder loads
     gate = _binary_mask(R, n, 1, H, W) if f["gate"] else None
+    if gate is not None and gate_nan:  # NaN < 0.5 is false: a NaN gate masks the pixel, as `image * (mask < 0.5)` does
+        gate = torch.where(R.rand(n, 1, H, W) < 0.05, NAN, gate)
     rows = n * h * w
 
     def fresh():
@@ -523,10 +529,10 @@ def replay_nchw_to_nhwc(R, f):
     return errs + e + e2, (res if e else res2)
 
 
-def replay_nhwc_to_nchw_clamp(R, f):
+def replay_nhwc_to_nchw_clamp(R, f, values=None):
     from ladi_vton_b200 import lib
     n, c, h, w, xp, lo, hi = f["n"], f["c"], f["h"], f["w"], f["xp"], f["lo"], f["hi"]
-    x = R.poisoned(n * h * w, xp, R.randn(n * h * w, c) * 0.8, dtype=torch.float32)
+    x = R.poisoned(n * h * w, xp, R.randn(n * h * w, c) * 0.8 if values is None else values, dtype=torch.float32)
 
     def fresh():
         flat, o = _buf(R, n * c * h * w, torch.float32)
@@ -534,7 +540,7 @@ def replay_nhwc_to_nchw_clamp(R, f):
     runs = _twice(lambda b: lib.call("ladi_nhwc_f32_to_nchw_clamp", C.c_void_p(x.data_ptr()), n, c, h, w, xp, lo, hi, C.c_void_p(b["out"].data_ptr()),
                                      R.stream), fresh)
     errs = _tail_nan(runs[0]["flat"], n * c * h * w, "output") + _determinism(runs, ["flat"])
-    ref = x[:, :c].reshape(n, h, w, c).permute(0, 3, 1, 2).clamp(lo, hi).contiguous().view(-1)
+    ref = x[:, :c].reshape(n, h, w, c).permute(0, 3, 1, 2).clamp(lo, hi).contiguous().view(-1)  # torch.clamp keeps NaN
     e, res = _exact(runs[0]["out"], ref, "values")
     return errs + e, res
 
@@ -614,11 +620,13 @@ def replay_check_binarise(R, f):
     return errs, (0.0 if not errs else float("inf"), "bit-exact mask and flags" if not errs else errs[0])
 
 
-def replay_posterior_sample(R, f):
+def replay_posterior_sample(R, f, logvar=None):
+    """logvar: [rows, cz] values in place of the random ones (past both clamps); NaN must come out NaN, as torch.clamp keeps it."""
     from ladi_vton_b200 import lib
     mp, n, cz, h, w, scale = f["mp"], f["n"], f["cz"], f["h"], f["w"], f["scale"]
     rows = n * h * w
-    mom = R.poisoned(rows, mp, torch.cat([R.randn(rows, cz) * 3, R.rand(rows, cz) * 60 - 36], dim=1), dtype=torch.float32)  # logvar past both clamps
+    lv0 = R.rand(rows, cz) * 60 - 36 if logvar is None else logvar
+    mom = R.poisoned(rows, mp, torch.cat([R.randn(rows, cz) * 3, lv0], dim=1), dtype=torch.float32)  # logvar past both clamps
     noise = R.randn(n, cz, h, w)
     cnt = n * cz * h * w
 
@@ -633,22 +641,28 @@ def replay_posterior_sample(R, f):
     sn = torch.exp(0.5 * lv) * noise.double()
     r = (mean + sn) * scale
     bound = abs(scale) * (2.0 ** -23 * mean.abs() + (2.0 ** -22 + 2.0 ** -23) * sn.abs()) + 2.0 ** -23 * r.abs()
-    e, res = _worst(ratio(runs[0]["out"].view(n, cz, h, w), r, bound), ("image", "channel", "y", "x"))
+    y = runs[0]["out"].view(n, cz, h, w)
+    nan = torch.isnan(r)
+    if not torch.equal(torch.isnan(y), nan):
+        errs.append(f"NaN at {int(torch.isnan(y).sum())} outputs where the reference has {int(nan.sum())} (a NaN logvar must stay NaN)")
+    e, res = _worst(ratio(y.masked_fill(nan, 0.0), r.masked_fill(nan, 0.0), bound.masked_fill(nan, 1.0)), ("image", "channel", "y", "x"))
     return errs + e, res
 
 
 def _ddim_coefs(R, steps=3):
-    ab = torch.tensor([0.05, 0.3, 0.7, 0.95], dtype=torch.float64)  # alphas-cumprod of consecutive DDIM steps, noisy to clean
+    ab = torch.tensor([0.01, 0.02, 0.03, 0.05, 0.3, 0.7, 0.95], dtype=torch.float64)[-(steps + 1):]  # alphas-cumprod, noisy to clean
     rows = torch.zeros((steps, 8), dtype=torch.float64)
     rows[:, 0], rows[:, 1] = ab[:steps].rsqrt(), (1 - ab[:steps]).sqrt()
     rows[:, 2], rows[:, 3], rows[:, 4] = ab[1:steps + 1].sqrt(), (1 - ab[1:steps + 1] - 0.01).sqrt(), 0.1
     return rows.float().to(R.dev)
 
 
-def replay_ddim_cfg_step(R, f):
+def replay_ddim_cfg_step(R, f, start=0):
+    """Three consecutive calls from device step index `start`: with advance, rows start, start + 1, start + 2 of the coefficient table
+    and step_ptr = [s + 1, 0] after each; without, row `start` every time and step_ptr untouched."""
     from ladi_vton_b200 import lib
-    ep, inp, B, h, w, cfg, g = f["ep"], f["inp"], f["B"], f["h"], f["w"], f["cfg"], f["guidance"]
-    assert f["coef"] and f["step"] and f["advance"], "the pipeline's DDIM update reads the step counter and advances it"
+    ep, inp, B, h, w, cfg, g, adv = f["ep"], f["inp"], f["B"], f["h"], f["w"], f["cfg"], f["guidance"], f["advance"]
+    assert f["coef"] and f["step"], "the pipeline's DDIM update reads the step counter"
     hw, Bp = h * w, (2 * B if cfg else B)
     eu = R.randn(B * hw, 4)
     eps = torch.cat([eu, eu + 0.3 * R.randn(B * hw, 4)]) if cfg else eu  # conditional = unconditional + a smaller difference
@@ -656,23 +670,25 @@ def replay_ddim_cfg_step(R, f):
     x_init = R.randn(B, 4, h, w)
     uin_init = R.randn(Bp * hw, inp).bfloat16()
     uin_init[:, :4] = NAN
-    coef = _ddim_coefs(R)
+    coef = _ddim_coefs(R, start + 3)
     noise = R.randn(B, 4, h, w) if f["noise"] else None
     P = lambda t: C.c_void_p(t.data_ptr() if t is not None else 0)  # noqa: E731
     g32 = float(np.float32(g))
 
     def run(check):
         lat, uin = x_init.clone(), uin_init.clone()
-        step = torch.zeros(2, dtype=torch.int32, device=R.dev)
+        step = torch.tensor([start, 0], dtype=torch.int32, device=R.dev)
         errs, worst = [], (0.0, "")
-        for s in range(coef.shape[0]):
+        for k in range(3):
+            s = start + k if adv else start
             x_before = lat.clone()
-            lib.call("ladi_ddim_cfg_step", P(eps), ep, P(lat), P(uin), inp, B, h, w, cfg, g, P(coef), P(step), 1, P(noise), R.stream)
+            lib.call("ladi_ddim_cfg_step", P(eps), ep, P(lat), P(uin), inp, B, h, w, cfg, g, P(coef), P(step), adv, P(noise), R.stream)
             torch.cuda.synchronize()
             if not check:
                 continue
-            if step.tolist() != [s + 1, 0]:
-                errs.append(f"step {s}: step_ptr {step.tolist()}, expected [{s + 1}, 0] (grid-wide ticket over {-(-B * 4 * hw // 256)} CTAs)")
+            want_step = [s + 1, 0] if adv else [start, 0]
+            if step.tolist() != want_step:
+                errs.append(f"step {s}: step_ptr {step.tolist()}, expected {want_step} (grid-wide ticket over {-(-B * 4 * hw // 256)} CTAs)")
             e3 = eps[:, :4].double().view(Bp, h, w, 4).permute(0, 3, 1, 2)
             r, bound = ddim_expect(x_before.double(), e3[:B], e3[B:] if cfg else None, coef[s].double(), g32, cfg,
                                    noise.double() if noise is not None else None)
@@ -704,11 +720,13 @@ def _image_out_input(R, n, h, w, xp):
     return R.poisoned(n * h * w, xp, v, dtype=torch.float32)
 
 
-def replay_image_out(R, f, u8=False):
+def replay_image_out(R, f, u8=False, values=None):
+    """values: [n*h*w, 3] fp32 in place of the random ones.  NaN: image_out keeps it (torch.clamp); image_out_u8 writes 0."""
     from ladi_vton_b200 import lib
-    assert f["f32"] == 1, "the decoder hands fp32 images to the conversion"
-    n, h, w, xp = f["n"], f["h"], f["w"], f["xp"]
-    x = _image_out_input(R, n, h, w, xp)
+    n, h, w, xp, f32 = f["n"], f["h"], f["w"], f["xp"], f["f32"]
+    x = _image_out_input(R, n, h, w, xp) if values is None else R.poisoned(n * h * w, xp, values, dtype=torch.float32)
+    if not f32:
+        x = x.bfloat16()
     cnt = n * h * w * 3
     dt = torch.uint8 if u8 else torch.float32
 
@@ -716,12 +734,13 @@ def replay_image_out(R, f, u8=False):
         flat, o = _buf(R, cnt, dt, fill=171 if u8 else NAN)
         return dict(flat=flat, out=o)
     name = "ladi_image_out_u8" if u8 else "ladi_image_out"
-    runs = _twice(lambda b: lib.call(name, C.c_void_p(x.data_ptr()), 1, n, h, w, xp, C.c_void_p(b["out"].data_ptr()), R.stream), fresh)
+    runs = _twice(lambda b: lib.call(name, C.c_void_p(x.data_ptr()), f32, n, h, w, xp, C.c_void_p(b["out"].data_ptr()), R.stream), fresh)
     tail = runs[0]["flat"][cnt:]
     errs = ([] if bool((tail == 171).all() if u8 else torch.isnan(tail).all()) else ["output: wrote past its end"]) + _determinism(runs, ["flat"])
-    c = (x[:, :3] * 0.5 + 0.5).clamp(0.0, 1.0)
+    c = (x[:, :3].float() * 0.5 + 0.5).clamp(0.0, 1.0)
     if u8:
-        ref = torch.from_numpy(np.rint(c.cpu().numpy() * np.float32(255.0)).astype(np.uint8)).to(R.dev)  # numpy: round half to even
+        v = np.rint(c.cpu().numpy() * np.float32(255.0))  # numpy: round half to even
+        ref = torch.from_numpy(np.where(np.isnan(v), 0.0, v).astype(np.uint8)).to(R.dev)
     else:
         ref = c
     e, res = _exact(runs[0]["out"].view(n * h * w, 3), ref.contiguous(), "values")
@@ -741,6 +760,8 @@ def replay_resize_aa(R, f):
                   fresh)
     out = runs[0]["out"].view(rows, op)
     errs = _window(out, c_off, c_off + c, "output") + _tail_nan(runs[0]["flat"], rows * op, "output") + _determinism(runs, ["flat"])
+    if (oh, ow) == (h, w):  # one tap of weight exactly 1 per output: bf16(x) bit for bit
+        errs += _exact(out[:, c_off:c_off + c].contiguous(), x.permute(0, 2, 3, 1).reshape(rows, c).bfloat16(), "identity resize")[0]
     worst = (0.0, "")
     for b in _pick(n, n * c * h * w, 1 << 24):
         r, bound = resample_expect(x[b].double(), oh, ow, U_BF16)
@@ -801,10 +822,11 @@ def _smooth_grid(R, n, gh, gw):
     return torch.stack([xs[None] + dx, ys[None] + dy], dim=3).contiguous()
 
 
-def replay_warp_grid_sample(R, f):
+def replay_warp_grid_sample(R, f, grid=None):
+    """grid: fp32 [n, gh, gw, 2] in place of the smooth TPS-like one."""
     from ladi_vton_b200 import lib
     gh, gw, n, c, H, W, op, c_off = (f[k] for k in ("gh", "gw", "n", "c", "H", "W", "op", "c_off"))
-    grid = _smooth_grid(R, n, gh, gw)
+    grid = _smooth_grid(R, n, gh, gw) if grid is None else grid.contiguous()
     cloth = _image(R, n, c, H, W)
     rows = n * H * W
 
@@ -867,10 +889,11 @@ def replay_space_to_depth2(R, f):
     return errs + e, res
 
 
-def replay_maxpool2(R, f):
+def replay_maxpool2(R, f, values=None):
+    """values: bf16 [n*h*w, c] in place of the post-ReLU features; a window holding a NaN gives NaN, as nn.MaxPool2d does."""
     from ladi_vton_b200 import lib
     n, h, w, c = f["n"], f["h"], f["w"], f["c"]
-    x = _features(R, n * h * w, c)
+    x = _features(R, n * h * w, c) if values is None else values.bfloat16().contiguous()
     cnt = n * (h // 2) * (w // 2) * c
 
     def fresh():
@@ -878,7 +901,7 @@ def replay_maxpool2(R, f):
         return dict(flat=flat, out=o)
     runs = _twice(lambda b: lib.call("ladi_maxpool2_nhwc", C.c_void_p(x.data_ptr()), n, h, w, c, C.c_void_p(b["out"].data_ptr()), R.stream), fresh)
     errs = _tail_nan(runs[0]["flat"], cnt, "output") + _determinism(runs, ["flat"])
-    ref = x.view(n, h // 2, 2, w // 2, 2, c).amax(dim=(2, 4)).reshape(-1)
+    ref = F.max_pool2d(x.view(n, h, w, c).permute(0, 3, 1, 2).float(), 2).permute(0, 2, 3, 1).bfloat16().reshape(-1)
     e, res = _exact(runs[0]["out"], ref.contiguous(), "values")
     return errs + e, res
 
@@ -968,10 +991,10 @@ def replay_channel_affine(R, f):
     return errs + e, res
 
 
-def replay_l2norm_channels(R, f):
+def replay_l2norm_channels(R, f, values=None):
     from ladi_vton_b200 import lib
     rows, c, pitch = f["rows"], f["c"], f["pitch"]
-    x0 = R.poisoned(rows, pitch, _features(R, rows, c))
+    x0 = R.poisoned(rows, pitch, _features(R, rows, c) if values is None else values)
 
     def fresh():
         return dict(x=x0.clone())
@@ -1022,9 +1045,13 @@ def replay_tps_grid(R, f):
     from ladi_vton_b200 import lib
     from ladi_vton_b200.warp import control_points, tps_matrices
     tp, n, nc, npts = f["tp"], f["n"], f["n_ctrl"], f["npts"]
-    assert nc == 25 and npts == 256 * 192, "replayed with the ConvNet_TPS(256, 192) matrices"
-    inv, rep = (t.to(R.dev).contiguous() for t in tps_matrices(256, 192, control_points()))
-    theta = R.poisoned(n, tp, torch.atanh(control_points().to(R.dev)).view(1, -1) + 0.2 * R.randn(n, 2 * nc), dtype=torch.float32)
+    if (nc, npts) == (25, 256 * 192):  # the ConvNet_TPS(256, 192) matrices
+        inv, rep = (t.to(R.dev).contiguous() for t in tps_matrices(256, 192, control_points()))
+        theta = R.poisoned(n, tp, torch.atanh(control_points().to(R.dev)).view(1, -1) + 0.2 * R.randn(n, 2 * nc), dtype=torch.float32)
+    else:  # other control-point and pixel counts: matrices of the same magnitudes
+        K = nc + 3
+        inv, rep = R.randn(K, K) * 2, torch.cat([R.rand(npts, K - 2) * 2 - 1, R.rand(npts, 2) * 2 - 1], dim=1)
+        theta = R.poisoned(n, tp, R.randn(n, 2 * nc), dtype=torch.float32)
 
     def fresh():
         pf, p = _buf(R, n * nc * 2, torch.float32)
