@@ -4,129 +4,11 @@ sequencing of the same kernels in ladi_vton_b200/{unet,vae,adapter}.py -- the se
 against the oracle.  The C++ side is walked in plan mode (no launches; `ladi_engine_trace`), the Python side runs on CPU tensors with
 the ABI calls recorded instead of executed (`lib.RECORD`).  Addresses differ (workspace offsets vs torch allocations), so both traces
 are normalised to (buffer id, byte offset) by data flow: a buffer is born where an op writes it, reads resolve to the youngest buffer
-containing the address, external operands (weights, inputs) are numbered by first appearance."""
-import re
-
+containing the address, external operands (weights, inputs) are numbered by first appearance (normalise in tests/kernel_check.py)."""
 import pytest
 import torch
 
-
-def _fmt_conv(d):
-    g = lambda a, i: int(a[i] or 0)
-    return (f"conv k={d.ksize} s={d.stride} p={d.pad_lo} up={d.up2x} n={d.n} h={d.h_out} w={d.w_out} hin={d.h_in} win={d.w_in} cout={d.c_out} nsrc={d.n_src} "
-            f"src0=@{g(d.src, 0):x} c0={d.src_c[0]} p0={d.src_pitch[0]} src1=@{g(d.src, 1):x} c1={d.src_c[1]} p1={d.src_pitch[1]} nsc={d.n_sc} "
-            f"sc0=@{g(d.sc, 0):x} sc0c={d.sc_c[0]} sc0p={d.sc_pitch[0]} sc1=@{g(d.sc, 1):x} sc1c={d.sc_c[1]} sc1p={d.sc_pitch[1]} "
-            f"wt=@{int(d.weight or 0):x} K={d.k_total} wp={d.weight_pitch} bias=@{int(d.bias or 0):x} bpr={d.bias_per_row} bss={d.bias_step_stride} "
-            f"step=@{int(d.step_ptr or 0):x} res=@{int(d.residual or 0):x} rp={d.residual_pitch} rs=@{int(d.row_scale or 0):x} act={d.act} "
-            f"out=@{int(d.out or 0):x} op={d.out_pitch} f32={d.out_fp32}")
-
-
-def _v(x):
-    return int(getattr(x, "value", x) or 0)
-
-
-def python_trace(records):
-    lines = []
-    for name, a in records:
-        if name == "ladi_conv2d_bf16":
-            lines.append(_fmt_conv(a[0]._obj))
-        elif name == "ladi_groupnorm_stats":
-            lines.append(f"gn_stats x0=@{_v(a[0]):x} c0={a[1]} p0={a[2]} x1=@{_v(a[3]):x} c1={a[4]} p1={a[5]} n={a[6]} hw={a[7]} groups={a[8]}")
-        elif name == "ladi_groupnorm_apply":
-            lines.append(f"gn_apply x0=@{_v(a[0]):x} c0={a[1]} p0={a[2]} x1=@{_v(a[3]):x} c1={a[4]} p1={a[5]} n={a[6]} hw={a[7]} groups={a[8]} gamma=@{_v(a[10]):x} "
-                         f"beta=@{_v(a[11]):x} eps={a[12]:.3g} silu={a[13]} add=@{_v(a[14]):x} ap={a[15]} out=@{_v(a[16]):x} op={a[17]}")
-        elif name == "ladi_layernorm":
-            lines.append(f"ln x=@{_v(a[0]):x} xp={a[1]} rows={a[2]} c={a[3]} gamma=@{_v(a[4]):x} beta=@{_v(a[5]):x} eps={a[6]:.3g} out=@{_v(a[7]):x} op={a[8]}")
-        elif name in ("ladi_attention_bf16", "ladi_attention_d512_bf16"):
-            d = a[0]._obj
-            hd = 64 if name == "ladi_attention_bf16" else d.head_dim
-            lines.append(f"attn d={hd} batch={d.batch} heads={d.heads} nq={d.nq} nkv={d.nkv} q=@{int(d.q):x} qp={d.q_pitch} qbs={d.q_batch_stride} k=@{int(d.k):x} "
-                         f"kp={d.k_pitch} kbs={d.k_batch_stride} v=@{int(d.v):x} vp={d.v_pitch} vbs={d.v_batch_stride} out=@{int(d.out):x} op={d.out_pitch} "
-                         f"obs={d.out_batch_stride} scale={d.scale:.6g}")
-        elif name == "ladi_add_bf16":
-            lines.append(f"add a=@{_v(a[0]):x} b=@{_v(a[1]):x} out=@{_v(a[2]):x} count={a[3]}")
-        elif name == "ladi_upsample2x_nhwc":
-            lines.append(f"upsample2x x=@{_v(a[0]):x} n={a[1]} h={a[2]} w={a[3]} c={a[4]} out=@{_v(a[5]):x}")
-        elif name == "ladi_cls_attention":
-            lines.append(f"cls_attn q=@{_v(a[0]):x} qp={a[1]} kv=@{_v(a[2]):x} kvp={a[3]} batch={a[4]} tokens={a[5]} heads={a[6]} hd={a[7]} out=@{_v(a[9]):x} op={a[10]}")
-        else:
-            lines.append(f"{name} (layout / pointwise op outside the module bodies)")
-    return lines
-
-
-def _out_bytes(op, f):
-    """Bytes the op writes starting at its `out` address (for the data-flow normalisation)."""
-    i = lambda k: int(f[k])
-    if op == "conv":
-        return ((i("n") * i("h") * i("w") - 1) * i("op") + (i("cout") // (2 if i("act") == 2 else 1))) * (4 if i("f32") else 2)
-    if op == "gn_apply":
-        return ((i("n") * i("hw") - 1) * i("op") + i("c0") + i("c1")) * 2
-    if op == "ln":
-        return ((i("rows") - 1) * i("op") + i("c")) * 2
-    if op == "attn":
-        width = i("heads") * 64 if i("d") == 64 else i("d")
-        return ((i("batch") - 1) * i("obs") + (i("nq") - 1) * i("op") + width) * 2
-    if op == "add":
-        return i("count") * 2
-    if op == "upsample2x":
-        return i("n") * 4 * i("h") * i("w") * i("c") * 2
-    if op == "cls_attn":
-        return ((i("batch") - 1) * i("op") + i("heads") * i("hd")) * 2
-    return 0
-
-
-def normalise(lines):
-    """@address -> B<k>+off for buffers written inside the trace (youngest containing buffer), X<k> for external operands."""
-    live, ext, out, nbuf = [], {}, [], 0  # live: [(start, end, id)], youngest last
-    for ln in lines:
-        op = ln.split(" ", 1)[0]
-        f = dict(re.findall(r"(\w+)=(\S+)", ln))
-        w_addr = int(f["out"][1:], 16) if "out" in f else None
-
-        def resolve(a):
-            if a == 0:
-                return "NULL"
-            for s, e, k in reversed(live):
-                if s <= a < e:
-                    return f"B{k}+{a - s}"
-            if a not in ext:
-                ext[a] = len(ext)
-            return f"X{ext[a]}"
-        toks = []
-        for k, v in re.findall(r"(\w+)=(\S+)", ln):
-            if v.startswith("@"):
-                if k == "out":
-                    continue
-                toks.append(f"{k}={resolve(int(v[1:], 16))}")
-            else:
-                toks.append(f"{k}={v}")
-        if w_addr is not None:
-            size = _out_bytes(op, f)
-            # every write gives birth to a buffer (no op of the module bodies writes into a slice of a buffer born inside the trace); older
-            # buffers it overlaps are dead -- the C++ allocator re-uses freed workspace, torch never overlaps
-            live[:] = [(s, e, k) for s, e, k in live if e <= w_addr or s >= w_addr + size]
-            live.append((w_addr, w_addr + size, nbuf))
-            toks.append(f"out=B{nbuf}")
-            nbuf += 1
-        out.append(op + " " + " ".join(toks))
-    return out
-
-
-def compare(py_records, cpp_trace, what):
-    a = normalise(python_trace(py_records))
-    b = normalise([l for l in cpp_trace.splitlines() if l.strip()])
-    for i, (x, y) in enumerate(zip(a, b)):
-        assert x == y, f"{what}: op {i} differs\n  python: {x}\n  c++   : {y}"
-    assert len(a) == len(b), f"{what}: {len(a)} Python ops vs {len(b)} C++ ops"
-    return len(a)
-
-
-@pytest.fixture()
-def record():
-    from ladi_vton_b200 import lib
-    lib.RECORD = []
-    yield lib
-    lib.RECORD = None
+from kernel_check import compare, record  # noqa: F401  (record: a fixture)
 
 
 def _cpu_pack(model):

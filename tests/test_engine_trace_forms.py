@@ -1,49 +1,11 @@
 """CPU test (no GPU needed): the launch sequences of the linear and 1x1 EMASC forms and of the inversion adapter with L > 1 encoder layers
 (csrc/engine.cu emasc_forward / adapter_forward, forms derived from the weight table) equal the Python sequencing of the same kernels in
-ladi_vton_b200/{vae,adapter}.py, op by op and operand by operand.  Same method as tests/test_engine_trace.py (its trace formatter and
-data-flow normalisation, extended here by the full-sequence attention of the extra adapter layers)."""
+ladi_vton_b200/{vae,adapter}.py, op by op and operand by operand.  Same method as tests/test_engine_trace.py, with the same trace formatter
+and data-flow normalisation (tests/kernel_check.py), which also format the full-sequence attention of the extra adapter layers."""
 import pytest
 import torch
 
-import test_engine_trace as base
-
-
-def _python_trace(records):
-    lines = []
-    for name, a in records:
-        if name == "ladi_attention_small":
-            v = [base._v(t) for t in a]
-            lines.append(f"attn_small batch={a[4]} heads={a[5]} nq={a[6]} nkv={a[7]} hd={a[8]} q=@{v[0]:x} qp={a[9]} qbs={a[13]} k=@{v[1]:x} "
-                         f"kp={a[10]} kbs={a[14]} v=@{v[2]:x} vp={a[11]} vbs={a[15]} out=@{v[3]:x} op={a[12]} obs={a[16]} scale={a[17]:.6g} "
-                         f"causal={a[18]}")
-        else:
-            lines += _base_python_trace([(name, a)])
-    return lines
-
-
-def _out_bytes(op, f):
-    if op == "attn_small":
-        i = lambda k: int(f[k])
-        return ((i("batch") - 1) * i("obs") + (i("nq") - 1) * i("op") + i("heads") * i("hd")) * 2
-    return _base_out_bytes(op, f)
-
-
-_base_python_trace, _base_out_bytes = base.python_trace, base._out_bytes
-
-
-@pytest.fixture()
-def compare(monkeypatch):
-    monkeypatch.setattr(base, "python_trace", _python_trace)
-    monkeypatch.setattr(base, "_out_bytes", _out_bytes)
-    return base.compare
-
-
-@pytest.fixture()
-def record():
-    from ladi_vton_b200 import lib
-    lib.RECORD = []
-    yield lib
-    lib.RECORD = None
+from kernel_check import compare, record  # noqa: F401  (record: a fixture)
 
 
 def _emasc(ein, eout, seed, **kw):
@@ -56,7 +18,7 @@ def _emasc(ein, eout, seed, **kw):
 
 
 @pytest.mark.parametrize("form", [dict(type="linear", padding=1), dict(kernel_size=1, padding=0), dict(kernel_size=3, padding=1)])
-def test_emasc_forms_sequence_matches_python(record, compare, form):
+def test_emasc_forms_sequence_matches_python(record, form):
     from ladi_vton_b200 import engine as eng, synthetic as S
     ein, eout = S.emasc_channels(S.SMALL_VAE["block_out_channels"])
     em = _emasc(ein, eout, 3, **form)
@@ -84,7 +46,7 @@ def test_emasc_engine_rejects_unknown_kernel_width():
 
 
 @pytest.mark.parametrize("L", [2, 3])
-def test_adapter_layers_sequence_matches_python(record, compare, L):
+def test_adapter_layers_sequence_matches_python(record, L):
     from ladi_vton_b200 import InversionAdapter, engine as eng, synthetic as S
     ad = InversionAdapter(input_dim=128, hidden_dim=256, output_dim=512, heads=2, mlp_dim=256, num_encoder_layers=L)
     ad._sd = S.random_state_dict(ad.param_shapes(), 4)
@@ -97,7 +59,7 @@ def test_adapter_layers_sequence_matches_python(record, compare, L):
     assert n == 12 + 7 * (L - 1)
 
 
-def test_adapter_one_layer_trace_unchanged(record, compare):
+def test_adapter_one_layer_trace_unchanged(record):
     """L = 1: no `adapter.enc*` weights, so the trace is the CLS-only sequence the release checkpoints run."""
     from ladi_vton_b200 import InversionAdapter, engine as eng, synthetic as S
     ad = InversionAdapter(input_dim=128, hidden_dim=256, output_dim=512, heads=2, mlp_dim=256, num_encoder_layers=1)

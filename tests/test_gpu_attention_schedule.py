@@ -1,6 +1,6 @@
 """The head-width-64 attention kernel at the edges of its schedule: the QK^T pipeline's prologue and drain (1, 2, 3, 4 and 24 key tiles),
 ragged last key tiles, query tails that leave some consumer warpgroups of the last query tile with few or no rows, and the fused-QKV
-projection read in place.  Each case is checked the way tests/test_gpu_workload_census.py checks the workload's calls: against float64
+projection read in place.  Each case is checked the way the workload census checks the workload's calls (tests/kernel_check.py): against float64
 with the same per-element bound, bit for bit against a second run, and with every byte of the output buffer outside the rows and columns
 the call owns (pitch gaps, the gap between batch images) NaN-poisoned before the call and still NaN after it."""
 import ctypes as C
@@ -8,7 +8,7 @@ import ctypes as C
 import pytest
 import torch
 
-from test_gpu_workload_census import Replay, _attn_ref, _bitwise_equal, attn_expect, ratio
+from kernel_check import Replay, attn_expect, attn_ref, max_ratio, same
 
 SCALE = 0.125
 PAD = 24  # columns of NaN after each row of every operand (keeps the pitch a multiple of 8)
@@ -81,11 +81,11 @@ def run_case(R, B, heads, nq, nkv, fused=False, D=64, late_max=False):
     owned.as_strided((B, nq, width), (obs, op, 1)).fill_(True)
     assert bool(torch.isfinite(out[owned].float()).all()), "unwritten or NaN-contaminated output element"
     assert bool(torch.isnan(out[~owned].float()).all()), "wrote outside its rows and columns (pitch gap or batch gap)"
-    assert _bitwise_equal(outs[0], outs[1]), "two runs differ bitwise"
+    assert same(outs[0], outs[1]), "two runs differ bitwise"
     ov = out.as_strided((B, nq, width), (obs, op, 1))
     for b in range(B):
-        o64, sv = _attn_ref(q[b].double(), k[b].double(), v[b].double(), heads, D, scale)
-        worst = float(ratio(ov[b], o64, attn_expect(o64, sv, nkv)).max())
+        o64, sv = attn_ref(q[b].double(), k[b].double(), v[b].double(), heads, D, scale)
+        worst = max_ratio(ov[b], o64, attn_expect(o64, sv, nkv))
         assert worst <= 1.0, f"image {b}: err/bound {worst:.3g}"
 
 

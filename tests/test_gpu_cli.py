@@ -10,13 +10,10 @@ import numpy as np
 import pytest
 import torch
 
+from kernel_check import rel_l2
+from model_pairs import NV, cli_models
+
 pytestmark = pytest.mark.gpu
-NV, CTX = 4, 128
-
-
-def rel_l2(y, ref):
-    y, ref = y.detach().float().cpu(), ref.detach().float().cpu()
-    return ((y - ref).norm() / ref.norm().clamp_min(1e-12)).item()
 
 
 @pytest.mark.parametrize("quantise", [False, True])
@@ -37,54 +34,9 @@ def test_clip_preprocess(cuda, quantise):
         ops.clip_preprocess(torch.zeros((1, 3, 2048, 64), device=cuda), 224, 224, mean, std)
 
 
-def _models(cuda):
-    """Engine modules + oracle twins on the same seeded weights."""
-    from test_gpu_frontend import _text_pair
-    from test_gpu_warp import _tps_pair, _unet_pair
-    from ladi_oracle.clip import ClipVisionEncoder
-    from ladi_oracle.parts import DDIMScheduler as ODDIM, EMASC as OEMASC, InversionAdapter as OAdapter
-    from ladi_oracle.pipeline import OracleTryOnPipeline
-    from ladi_oracle.unet import UNet2DConditionModel as OU
-    from ladi_oracle.vae import AutoencoderKL as OV
-    from ladi_vton_b200 import (EMASC, AutoencoderKL, CLIPVisionModelWithProjection, DDIMScheduler, InversionAdapter, UNet2DConditionModel,
-                                synthetic as S)
-    from ladi_vton_b200.inference import StandInTokenizer
-    text, otext = _text_pair(cuda, 21, vocab_size=49408, hidden_size=CTX, intermediate_size=256, num_hidden_layers=2, num_attention_heads=2)
-    vis = CLIPVisionModelWithProjection(hidden_size=160, intermediate_size=320, num_hidden_layers=2, num_attention_heads=2)
-    c = vis.config
-    vsd = S.random_state_dict(vis.param_shapes(), 31)
-    for k in vsd:
-        if "embedding" in k and "patch" not in k:
-            vsd[k] = torch.randn(vsd[k].shape, generator=torch.Generator().manual_seed(len(k)))
-    ovis = ClipVisionEncoder(dim=c.hidden_size, heads=c.num_attention_heads, layers=c.num_hidden_layers, mlp=c.intermediate_size,
-                             image=c.image_size, patch=c.patch_size).eval()
-    ovis.load_state_dict(vsd)
-    ad = InversionAdapter(input_dim=160, hidden_dim=256, output_dim=CTX * NV, heads=2, mlp_dim=320)
-    asd = S.random_state_dict(ad.param_shapes(), 41)
-    oad = OAdapter(input_dim=160, hidden_dim=256, output_dim=CTX * NV, heads=2, mlp_dim=320).eval()
-    oad.load_state_dict(asd)
-    tps, otps = _tps_pair(cuda)
-    ref, oref = _unet_pair(cuda)
-    sds = S.build_state_dicts(S.SMALL_UNET, S.SMALL_VAE, seed=5)
-    eng = dict(scheduler=DDIMScheduler(), text_encoder=text, vision_encoder=vis.load_state_dict(vsd).to(cuda),
-               inversion_adapter=ad.load_state_dict(asd).to(cuda), tps=tps, refinement=ref, tokenizer=StandInTokenizer(),
-               unet=UNet2DConditionModel(**S.SMALL_UNET).load_state_dict(sds["unet"]).to(cuda),
-               vae=AutoencoderKL(**S.SMALL_VAE).load_state_dict(sds["vae"]).to(cuda),
-               emasc=EMASC(*sds["emasc_channels"]).load_state_dict(sds["emasc"]).to(cuda))
-    ou = OU(**S.SMALL_UNET).eval()
-    ou.load_state_dict(sds["unet"])
-    ov = OV(**S.SMALL_VAE).eval()
-    ov.load_state_dict(sds["vae"])
-    oe = OEMASC(*sds["emasc_channels"]).eval()
-    oe.load_state_dict(sds["emasc"])
-    orc = dict(tps=otps, refinement=oref, vision_encoder=ovis, inversion_adapter=oad, tokenizer=StandInTokenizer(), text_encoder=otext,
-               pipe=OracleTryOnPipeline(ov, ou, ODDIM(), oe, [1, 2, 3, 4, 5]))
-    return eng, orc
-
-
 @pytest.fixture(scope="module")
 def models(cuda):
-    return _models(cuda)
+    return cli_models(cuda)
 
 
 ARGV = ["--test_order", "paired", "--dataset", "vitonhd", "--synthetic_samples", "3", "--batch_size", "2", "--num_inference_steps", "2",

@@ -3,7 +3,7 @@
 `ladi_conv2d_plan` reports the plan `ladi_conv2d_bf16` runs for a descriptor (N tile, split-K factor, CTA pairs, staged or fragment
 epilogue, pipeline stages, tile grid), from the same code that launches it.  Every GPU case below first asserts the plan it means to
 exercise -- N tile, splits, pair, store path, and the work-item count relative to the device's SM count -- and then runs the call the way
-tests/test_gpu_workload_census.py replays the workloads: input pitch gaps NaN, the output NaN over its full pitch plus tail rows, every
+the workload census replays the workloads (tests/kernel_check.py): input pitch gaps NaN, the output NaN over its full pitch plus tail rows, every
 owned element finite and every other still NaN afterwards, a second run bit-identical, and every element within the census's per-element
 float64 bound (conv_expect / ratio).
 
@@ -27,11 +27,11 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from test_gpu_workload_census import C_ACC, EPS24, _attn_ref, attn_expect, conv_expect, ratio
+from kernel_check import (C_ACC, EPS24, TAIL, addr, attn_expect, attn_ref, conv_expect, cpu_gen, determinism, ladi_lib, layout, max_ratio, nan_buf,
+                          plan_query, same, sms, twice)
 
 FORMS = ["bias", "nobias", "stepbias", "rowbias", "silu", "gelu", "relu", "geglu", "residual", "inplace", "rowscale", "fp32"]
 SPLIT_FORMS = ["nobias", "bias", "stepbias", "silu", "gelu", "relu", "residual", "inplace"]
-TAIL = 3  # NaN rows after the output that no call may write
 
 
 # ================================================================================================================ float64 expectations
@@ -89,46 +89,32 @@ def ln_fold_expect(t, wp, colsum, bp, eps, act=0):
     return conv_expect(pre, e / (C_ACC * math.sqrt(C_) * EPS24), C_, act)
 
 
-def worst(y, r, bound):
-    return float(ratio(y, r, bound).max())
-
-
 # ================================================================================================================ CPU: the plan table
-def _lib():
-    from ladi_vton_b200 import lib
-    return lib
-
-
-BASE = 1 << 40  # fake device addresses: the query dereferences nothing
-
-
-def _addr(slot, byte_off=0):
-    return BASE + slot * (1 << 32) + byte_off
 
 
 def gemm_desc(M, K, N, **kw):
     """A GEMM descriptor on fake, 256-byte aligned addresses; kw overrides fields (pointer fields take byte offsets via *_off)."""
-    lib = _lib()
+    lib = ladi_lib()
     d = lib.ConvDesc()
     d.n, d.h_out, d.w_out, d.c_out = 1, 1, M, N
     d.ksize, d.stride, d.pad_lo = 1, 1, 0
-    d.n_src, d.src[0], d.src_c[0], d.src_pitch[0] = 1, _addr(1), K, (K + 7) // 8 * 8
+    d.n_src, d.src[0], d.src_c[0], d.src_pitch[0] = 1, addr(1), K, (K + 7) // 8 * 8
     kt = (K + 63) // 64 * 64
-    d.weight, d.k_total, d.weight_pitch = _addr(2), kt, kt
-    d.out, d.out_pitch = _addr(3), N
+    d.weight, d.k_total, d.weight_pitch = addr(2), kt, kt
+    d.out, d.out_pitch = addr(3), N
     return _fill(d, kw)
 
 
 def conv_desc(n, h, w, cin, cout, k=3, s=1, **kw):
-    lib = _lib()
+    lib = ladi_lib()
     d = lib.ConvDesc()
     d.n, d.h_out, d.w_out, d.c_out = n, h, w, cout
     d.h_in, d.w_in = h * s, w * s
     d.ksize, d.stride, d.pad_lo = k, s, 1 if k == 3 else 0
-    d.n_src, d.src[0], d.src_c[0], d.src_pitch[0] = 1, _addr(1), cin, (cin + 7) // 8 * 8
+    d.n_src, d.src[0], d.src_c[0], d.src_pitch[0] = 1, addr(1), cin, (cin + 7) // 8 * 8
     kt = k * k * ((cin + 63) // 64 * 64)
-    d.weight, d.k_total, d.weight_pitch = _addr(2), kt, kt
-    d.out, d.out_pitch = _addr(3), cout
+    d.weight, d.k_total, d.weight_pitch = addr(2), kt, kt
+    d.out, d.out_pitch = addr(3), cout
     return _fill(d, kw)
 
 
@@ -137,9 +123,9 @@ def _fill(d, kw):
     for key, v in kw.items():
         if key.endswith("_off"):
             name = key[:-4]
-            setattr(d, name, (getattr(d, name) or _addr(slots[name])) + v)
+            setattr(d, name, (getattr(d, name) or addr(slots[name])) + v)
         elif key in slots and v is True:
-            setattr(d, key, _addr(slots[key]))
+            setattr(d, key, addr(slots[key]))
         else:
             setattr(d, key, v)
     if d.splitk_ws and not d.splitk_ws_bytes:
@@ -150,16 +136,14 @@ def _fill(d, kw):
 
 
 def plan_of(d, sms):
-    p = _lib().conv_plan(d, sms)
+    p = ladi_lib().conv_plan(d, sms)
     return dict(bn=p.bn, splits=p.splits, per=p.kb_per_split, pair=bool(p.pair), staged=bool(p.staged), stages=p.stages,
                 tiles_m=p.tiles_m, tiles_n=p.tiles_n, kb=p.total_kb, items=p.items())
 
 
 def rejected(d, sms=132):
-    lib = _lib().load()
-    plan = _lib().ConvPlan()
-    rc = lib.ladi_conv2d_plan(C.byref(d), sms, C.byref(plan))
-    return (rc, lib.ladi_last_error().decode()) if rc else (0, "")
+    p, err = plan_query("ladi_conv2d_plan", ladi_lib().ConvPlan, [C.byref(d), sms], ())
+    return (0, "") if p is not None else (1, err)
 
 
 no_env_pairs = pytest.mark.skipif(os.environ.get("LADI_CONV_2CTA") == "1", reason="LADI_CONV_2CTA=1 changes the library default")
@@ -291,13 +275,13 @@ def test_placement_rules_statistics(what):
 
 
 def _attn_desc(**kw):
-    lib = _lib()
+    lib = ladi_lib()
     d = lib.AttnDesc()
     d.batch, d.heads, d.nq, d.nkv = 2, 2, 100, 77
-    d.q, d.q_pitch, d.q_batch_stride = _addr(1), 128, 128 * 100
-    d.k, d.k_pitch, d.k_batch_stride = _addr(2), 128, 128 * 77
-    d.v, d.v_pitch, d.v_batch_stride = _addr(3), 128, 128 * 77
-    d.out, d.out_pitch, d.out_batch_stride = _addr(4), 128, 128 * 100
+    d.q, d.q_pitch, d.q_batch_stride = addr(1), 128, 128 * 100
+    d.k, d.k_pitch, d.k_batch_stride = addr(2), 128, 128 * 77
+    d.v, d.v_pitch, d.v_batch_stride = addr(3), 128, 128 * 77
+    d.out, d.out_pitch, d.out_batch_stride = addr(4), 128, 128 * 100
     d.scale = 0.125
     for k, v in kw.items():
         setattr(d, k, v)
@@ -312,7 +296,7 @@ ATTN_REJECT = {"out 2-byte aligned": ("out", "out"), "odd out_batch_stride": ("o
 @pytest.mark.parametrize("name", list(ATTN_REJECT))
 def test_attention_placement_rejected(entry, name):
     """Both entry points validate before they touch a device, so the rejection is visible here."""
-    lib = _lib().load()
+    lib = ladi_lib().load()
     field, word = ATTN_REJECT[name]
     if entry == "ladi_attention_d512_bf16":
         cols = 512
@@ -380,7 +364,7 @@ def test_gemm_checker_accepts_honest_schedule():
     a, w, b, acc, m = _tile_case(5)
     r, bound = gemm_expect(acc, m, a.shape[1], bcol=b.double())
     for splits in (1, 3, 10):
-        assert worst(_emulate_tiles(a, w, b, splits=splits), r, bound) <= 1.0
+        assert max_ratio(_emulate_tiles(a, w, b, splits=splits), r, bound) <= 1.0
 
 
 @pytest.mark.parametrize("fault,splits", [("drop_last_kb", 1), ("tile_shift", 1), ("split_twice", 3), ("phantom", 1)])
@@ -389,8 +373,8 @@ def test_gemm_checker_rejects_schedule_faults(fault, splits):
     twice; 4. the phantom pair row stored into the last real tile."""
     a, w, b, acc, m = _tile_case(6)
     r, bound = gemm_expect(acc, m, a.shape[1], bcol=b.double())
-    assert worst(_emulate_tiles(a, w, b, splits=splits), r, bound) <= 1.0
-    assert worst(_emulate_tiles(a, w, b, splits=splits, fault=fault), r, bound) > 1.0
+    assert max_ratio(_emulate_tiles(a, w, b, splits=splits), r, bound) <= 1.0
+    assert max_ratio(_emulate_tiles(a, w, b, splits=splits, fault=fault), r, bound) > 1.0
 
 
 def _ln_case(seed, M=96, Cin=320, N=192, mean=8.0):
@@ -428,8 +412,8 @@ def test_ln_checker_teeth():
     """5. the LayerNorm mean term dropped for one row: rejected; the honest fp32 emulation (mean 8 >> std 1): accepted."""
     t, wp, colsum, bp = _ln_case(7)
     r, bound = ln_fold_expect(t, wp, colsum, bp, 1e-5)
-    assert worst(_emulate_ln_consumer(t, wp, colsum, bp, 1e-5), r, bound) <= 1.0
-    assert worst(_emulate_ln_consumer(t, wp, colsum, bp, 1e-5, drop_mean_row=17), r, bound) > 1.0
+    assert max_ratio(_emulate_ln_consumer(t, wp, colsum, bp, 1e-5), r, bound) <= 1.0
+    assert max_ratio(_emulate_ln_consumer(t, wp, colsum, bp, 1e-5, drop_mean_row=17), r, bound) > 1.0
 
 
 def test_rowstat_checker_teeth():
@@ -442,25 +426,19 @@ def test_rowstat_checker_teeth():
     s, q, bs, bq = rowstat_expect(pre + res, e)
     y32 = (a.float() @ w.float().t() + b) + res.float()
     honest = _stats_table(y32)
-    assert worst(honest[..., 0], s, bs) <= 1.0 and worst(honest[..., 1], q, bq) <= 1.0
+    assert max_ratio(honest[..., 0], s, bs) <= 1.0 and max_ratio(honest[..., 1], q, bq) <= 1.0
     bad = honest.clone()
     bad[5, 2] = honest[5, 3]
-    assert worst(bad[..., 0], s, bs) > 1.0 or worst(bad[..., 1], q, bq) > 1.0
+    assert max_ratio(bad[..., 0], s, bs) > 1.0 or max_ratio(bad[..., 1], q, bq) > 1.0
 
 
 # ================================================================================================================ GPU
-def _sms(dev):
-    return torch.cuda.get_device_properties(dev).multi_processor_count
-
-
-def _gen(seed):
-    return torch.Generator(device="cpu").manual_seed(seed)
 
 
 def _operands(form, rows, c_out, c_eff, dev, seed):
     """(ops kwargs, column bias, row bias, residual bf16 [rows, c_eff], row scale, act, fp32 out) of one epilogue form; float64 copies."""
     from ladi_vton_b200 import ops
-    g = _gen(seed)
+    g = cpu_gen(seed)
     act = {"silu": ops.ACT_SILU, "gelu": ops.ACT_GELU, "relu": ops.ACT_RELU, "geglu": ops.ACT_GEGLU}.get(form, ops.ACT_NONE)
     kw, bcol, brow, res, rs = {"act": act}, None, None, None, None
     if form == "stepbias":  # the engine's per-step tables: the row of step 2, at an offset into the table
@@ -484,28 +462,12 @@ def _operands(form, rows, c_out, c_eff, dev, seed):
     return kw, bcol, brow, res, rs, act, form == "fp32"
 
 
-def _nan(shape, dtype, dev):
-    return torch.full(shape, float("nan"), dtype=dtype, device=dev)
-
-
-def _layout_ok(buf, rows, cols):
-    o = buf.float()
-    assert bool(torch.isfinite(o[:rows, :cols]).all()), f"unwritten or NaN-tainted output at {(~torch.isfinite(o[:rows, :cols])).nonzero()[0].tolist()}"
-    outside = torch.ones_like(o, dtype=torch.bool)
-    outside[:rows, :cols] = False
-    assert bool(torch.isnan(o[outside]).all()), "the call wrote outside its output"
-
-
-def _bits(t):
-    return t.view({torch.bfloat16: torch.int16, torch.float32: torch.int32}[t.dtype])
-
-
 def run_gemm(dev, M, K, N, form="bias", out_pitch=None, expect=None, seed=0, **kw):
     """One GEMM through ops.gemm as described in the module docstring; `expect(plan)` asserts the plan first.  -> (plan, output)."""
     from ladi_vton_b200 import ops, weights
-    g = _gen(seed)
+    g = cpu_gen(seed)
     c_eff = N // 2 if form == "geglu" else N
-    abuf = _nan((M, K + 8), torch.bfloat16, dev)
+    abuf = nan_buf((M, K + 8), torch.bfloat16, dev)
     abuf[:, :K] = torch.randn((M, K), generator=g).to(dev).bfloat16()
     a = abuf[:, :K]
     w = (torch.randn((N, K), generator=g) * K ** -0.5).bfloat16()
@@ -516,11 +478,11 @@ def run_gemm(dev, M, K, N, form="bias", out_pitch=None, expect=None, seed=0, **k
     pitch = out_pitch or c_eff + 8
     rbuf = None
     if res is not None and form != "inplace":
-        rbuf = _nan((M, pitch), torch.bfloat16, dev)
+        rbuf = nan_buf((M, pitch), torch.bfloat16, dev)
         rbuf[:, :c_eff] = res
 
     def fresh():
-        buf = _nan((M + TAIL, pitch), odt, dev)
+        buf = nan_buf((M + TAIL, pitch), odt, dev)
         if form == "inplace":
             buf[:M, :c_eff] = res
             return buf, buf[:M, :c_eff]
@@ -530,18 +492,16 @@ def run_gemm(dev, M, K, N, form="bias", out_pitch=None, expect=None, seed=0, **k
     plan = ops.gemm_plan(a, wp, N, out=buf[:M, :c_eff], residual=resid, out_fp32=f32, **okw)
     if expect is not None:
         expect(plan)
-    outs = []
-    for _ in range(2):
-        buf, resid = fresh()
-        ops.gemm(a, wp, N, out=buf[:M, :c_eff], residual=resid, out_fp32=f32, **okw)
-        outs.append(buf)
-    torch.cuda.synchronize()
-    _layout_ok(outs[0], M, c_eff)
-    assert torch.equal(_bits(outs[0]), _bits(outs[1])), "two runs differ bitwise"
+    runs = twice(lambda b: ops.gemm(a, wp, N, out=b["out"][:M, :c_eff], residual=b["res"], out_fp32=f32, **okw),
+                 lambda: dict(zip(("out", "res"), fresh())))
+    outs = [r["out"] for r in runs]
+    errs = layout(outs[0], 0, c_eff, "output", rows=M)
+    assert not errs, errs
+    assert not determinism(runs, ["out"]), "two runs differ bitwise"
     acc = a.double() @ w.to(dev).double().t()
     m = a.double().abs() @ w.to(dev).double().abs().t()
     r, bound = gemm_expect(acc, m, K, bcol, brow, None if res is None else res.double(), rs, act, f32)
-    q = worst(outs[0][:M, :c_eff], r, bound)
+    q = max_ratio(outs[0][:M, :c_eff], r, bound)
     assert q <= 1.0, f"err/bound {q:.3g} (plan bn {plan.bn} splits {plan.splits} pair {plan.pair} staged {plan.staged})"
     return plan, outs[0][:M, :c_eff]
 
@@ -564,7 +524,7 @@ ITEM_COUNTS = {"1": lambda s: 1, "2": lambda s: 2, "sms-1": lambda s: s - 1, "sm
 def test_items_vs_sms(cuda, path, items):
     """Work items around the persistent grid: a CTA's last item, one item per CTA, one CTA taking a second item, and (pairs) more pairs
     than co-resident clusters.  The last M tile is ragged; pairs run an odd M-tile count (a phantom tile) except at 1 item."""
-    T = ITEM_COUNTS[items](_sms(cuda))
+    T = ITEM_COUNTS[items](sms(cuda))
     if path == "pair128":
         tiles_m = 2 if T == 1 else 2 * T - 1
         M, N, kw = 128 * tiles_m - 40, 128, dict(force_bn=128, pair=True)
@@ -592,10 +552,10 @@ def test_k_depth(cuda, path, items, depth):
     from ladi_vton_b200 import lib
     bn, staged = PATHS[path]
     pitch = bn + 8 if staged else bn + 4  # c_out + 4: rows are not whole 16-byte chunks -> fragment stores
-    stages = lib.conv_plan(gemm_desc(1000, 64, bn, force_bn=bn, out_pitch=pitch), _sms(cuda)).stages
+    stages = lib.conv_plan(gemm_desc(1000, 64, bn, force_bn=bn, out_pitch=pitch), sms(cuda)).stages
     assert stages == {32: 8, 64: 8, 128: 6 if staged else 7, 160: 6, 192: 5, 256: 4}[bn]
     kb = DEPTHS[depth](stages)
-    T = 1 if items == "1" else _sms(cuda) + 1
+    T = 1 if items == "1" else sms(cuda) + 1
     run_gemm(cuda, 128 * T - 24, 64 * kb, bn, form="bias", out_pitch=pitch, force_bn=bn, seed=kb,
              expect=_want(bn=bn, staged=int(staged), stages=stages, total_kb=kb, splits=1, pair=0, items=T))
 
@@ -614,7 +574,7 @@ def _split_shape(plan_name, sms):
 @pytest.mark.parametrize("form", SPLIT_FORMS)
 @pytest.mark.parametrize("plan_name", ["S2", "ragged", "S16"])
 def test_split_k(cuda, plan_name, form):
-    M, K, N = _split_shape(plan_name, _sms(cuda))
+    M, K, N = _split_shape(plan_name, sms(cuda))
 
     def expect(plan):
         S, per, kb = plan.splits, plan.kb_per_split, plan.total_kb
@@ -646,7 +606,7 @@ def test_pair_matches_single(cuda, bn):
     M, K, N = 7 * 128 - 5, 9 * 64, 2 * bn + 64
     _, y2 = run_gemm(cuda, M, K, N, form="residual", force_bn=bn, pair=True, seed=3, expect=_want(bn=bn, pair=1, tiles_m=7, items=4 * 3))
     _, y1 = run_gemm(cuda, M, K, N, form="residual", force_bn=bn, pair=False, seed=3, expect=_want(bn=bn, pair=0))
-    assert torch.equal(_bits(y1), _bits(y2)), "paired and single CTAs differ"
+    assert same(y1, y2), "paired and single CTAs differ"
 
 
 # ---------------------------------------------------------------------------------------------------------------- convolutions
@@ -656,10 +616,10 @@ def run_conv(dev, n, hin, win, cins, cout, *, k=3, s=1, pad_lo=1, scs=(), form="
     up2x: weights are multiples of 1/64 below 1/8, so the merged sub-pixel taps are exact and the reference is the convolution of the
     nearest-upsampled input."""
     from ladi_vton_b200 import ops, weights
-    g = _gen(seed)
+    g = cpu_gen(seed)
     xs = []
     for c in cins:
-        b = _nan((n, hin, win, c + 8), torch.bfloat16, dev)
+        b = nan_buf((n, hin, win, c + 8), torch.bfloat16, dev)
         b[..., :c] = torch.randn((n, hin, win, c), generator=g).to(dev).bfloat16()
         xs.append(b[..., :c])
     if up2x:
@@ -671,7 +631,7 @@ def run_conv(dev, n, hin, win, cins, cout, *, k=3, s=1, pad_lo=1, scs=(), form="
         h, w = hin, win
     sc = []
     for c in scs:
-        b = _nan((n, h, w, c + 8), torch.bfloat16, dev)
+        b = nan_buf((n, h, w, c + 8), torch.bfloat16, dev)
         b[..., :c] = torch.randn((n, h, w, c), generator=g).to(dev).bfloat16()
         sc.append(b[..., :c])
     cin, csc = sum(cins), sum(scs)
@@ -691,27 +651,24 @@ def run_conv(dev, n, hin, win, cins, cout, *, k=3, s=1, pad_lo=1, scs=(), form="
     pitch = cout + 8
     rbuf = None
     if res is not None:
-        rbuf = _nan((rows, pitch), torch.bfloat16, dev)
+        rbuf = nan_buf((rows, pitch), torch.bfloat16, dev)
         rbuf[:, :cout] = res
     common = dict(ksize=k, stride=s, pad_lo=pad_lo, shortcut=sc, up2x=up2x, out_fp32=f32, **okw)
 
     def views(buf):
         return buf[:rows].view(n, h, w, pitch)[..., :cout], None if rbuf is None else rbuf.view(n, h, w, pitch)[..., :cout]
 
-    buf = _nan((rows + TAIL, pitch), odt, dev)
+    buf = nan_buf((rows + TAIL, pitch), odt, dev)
     o4, r4 = views(buf)
     plan = ops.conv_plan(xs, wp.to(dev), cout, out=o4, residual=r4, **common)
     if expect is not None:
         expect(plan)
-    outs = []
-    for _ in range(2):
-        buf = _nan((rows + TAIL, pitch), odt, dev)
-        o4, r4 = views(buf)
-        ops.conv2d(xs, wp.to(dev), cout, out=o4, residual=r4, **common)
-        outs.append(buf)
-    torch.cuda.synchronize()
-    _layout_ok(outs[0], rows, cout)
-    assert torch.equal(_bits(outs[0]), _bits(outs[1])), "two runs differ bitwise"
+    runs = twice(lambda b: ops.conv2d(xs, wp.to(dev), cout, out=views(b["out"])[0], residual=views(b["out"])[1], **common),
+                 lambda: dict(out=nan_buf((rows + TAIL, pitch), odt, dev)))
+    outs = [r["out"] for r in runs]
+    errs = layout(outs[0], 0, cout, "output", rows=rows)
+    assert not errs, errs
+    assert not determinism(runs, ["out"]), "two runs differ bitwise"
     X = torch.cat([x.double() for x in xs], dim=3).permute(0, 3, 1, 2)
     if up2x:
         X = F.interpolate(X, scale_factor=2, mode="nearest")
@@ -728,7 +685,7 @@ def run_conv(dev, n, hin, win, cins, cout, *, k=3, s=1, pad_lo=1, scs=(), form="
         m += S_.abs() @ wsc.to(dev).double().abs().t()
     K = wp.shape[1]
     r, bound = gemm_expect(acc, m, K, bcol, brow, None if res is None else res.double(), rs, act, f32)
-    q = worst(outs[0][:rows, :cout], r, bound)
+    q = max_ratio(outs[0][:rows, :cout], r, bound)
     assert q <= 1.0, f"err/bound {q:.3g}"
     return plan
 
@@ -761,7 +718,7 @@ def test_rowstat_producer(cuda, form):
     rows of mean 8: the statistics of a tensor whose mean dwarfs its spread)."""
     from ladi_vton_b200 import ops, weights
     M, K, N = 1000, 320, 320
-    g = _gen(31)
+    g = cpu_gen(31)
     a = torch.randn((M, K), generator=g).to(cuda).bfloat16()
     w = (torch.randn((N, K), generator=g) * K ** -0.5).bfloat16()
     wp = weights.pack_linear(w.float()).to(cuda)
@@ -769,7 +726,7 @@ def test_rowstat_producer(cuda, form):
     res = (torch.randn((M, N), generator=g) + 8).to(cuda).bfloat16() if form == "residual" else None
     act = ops.ACT_SILU if form == "silu" else ops.ACT_NONE
     stats = torch.full((M, N // 32, 2), float("nan"), device=cuda)
-    out = _nan((M, N + 8), torch.bfloat16, cuda)
+    out = nan_buf((M, N + 8), torch.bfloat16, cuda)
     plan = ops.gemm_plan(a, wp, N, bias=b, residual=res, act=act, out=out[:, :N], rowstat=stats, split_k=False)
     assert plan.staged == 0 and plan.splits == 1
     ops.gemm(a, wp, N, bias=b, residual=res, act=act, out=out[:, :N], rowstat=stats, split_k=False)
@@ -778,10 +735,10 @@ def test_rowstat_producer(cuda, form):
     m = a.double().abs() @ w.to(cuda).double().abs().t()
     r64 = None if res is None else res.double()
     r, bound = gemm_expect(acc, m, K, bcol=b.double(), res=r64, act=act)
-    assert worst(out[:, :N], r, bound) <= 1.0
+    assert max_ratio(out[:, :N], r, bound) <= 1.0
     s, q, bs, bq = rowstat_expect(r, bound - 2.0 ** -7 * r.abs())
-    assert worst(stats[..., 0], s, bs) <= 1.0, "row sums"
-    assert worst(stats[..., 1], q, bq) <= 1.0, "row sums of squares"
+    assert max_ratio(stats[..., 0], s, bs) <= 1.0, "row sums"
+    assert max_ratio(stats[..., 1], q, bq) <= 1.0, "row sums of squares"
 
 
 @pytest.mark.gpu
@@ -797,17 +754,18 @@ def test_ln_fold_consumer(cuda, act, bn):
     c_eff = N // 2 if act == "geglu" else N
     stats = _stats_table(t.float()).to(cuda)
     eps = 1e-5
-    tbuf = _nan((M, Cin + 8), torch.bfloat16, cuda)
+    tbuf = nan_buf((M, Cin + 8), torch.bfloat16, cuda)
     tbuf[:, :Cin] = t
-    out = _nan((M + TAIL, c_eff + 8), torch.bfloat16, cuda)
+    out = nan_buf((M + TAIL, c_eff + 8), torch.bfloat16, cuda)
     kw = dict(bias=bp, act=a_code, ln=(stats, colsum, eps), force_bn=bn, split_k=False)
     plan = ops.gemm_plan(tbuf[:, :Cin], wp, N, out=out[:M, :c_eff], **kw)
     assert plan.staged == 0 and plan.splits == 1 and (bn == 0 or plan.bn == bn)
     ops.gemm(tbuf[:, :Cin], wp, N, out=out[:M, :c_eff], **kw)
     torch.cuda.synchronize()
-    _layout_ok(out, M, c_eff)
+    errs = layout(out, 0, c_eff, "output", rows=M)
+    assert not errs, errs
     r, bound = ln_fold_expect(t, wp, colsum, bp, eps, a_code)
-    q = worst(out[:M, :c_eff], r, bound)
+    q = max_ratio(out[:M, :c_eff], r, bound)
     assert q <= 1.0, f"err/bound {q:.3g}"
 
 
@@ -836,8 +794,8 @@ def test_placement(cuda, path, operand, offset, parity):
     from ladi_vton_b200 import lib, ops, weights
     M, K, N, kw = PLACE_PATHS[path]
     pitch = N + 8 if parity == "even" else N + 3
-    g = _gen(offset * 7 + len(operand))
-    abuf = _nan((M, K + 8), torch.bfloat16, cuda)
+    g = cpu_gen(offset * 7 + len(operand))
+    abuf = nan_buf((M, K + 8), torch.bfloat16, cuda)
     abuf[:, :K] = torch.randn((M, K), generator=g).to(cuda).bfloat16()
     a = abuf[:, :K]
     w = (torch.randn((N, K), generator=g) * K ** -0.5).bfloat16()
@@ -847,10 +805,10 @@ def test_placement(cuda, path, operand, offset, parity):
     bstore[b_off:b_off + N] = (torch.randn((N,), generator=g) * 0.5).to(cuda)
     bias = bstore[b_off:b_off + N]
     res = torch.randn((M, N), generator=g).to(cuda).bfloat16()
-    rstore = _nan((M * pitch + 16,), torch.bfloat16, cuda)
+    rstore = nan_buf((M * pitch + 16,), torch.bfloat16, cuda)
     resid = rstore[r_off:r_off + M * pitch].view(M, pitch)[:, :N]
     resid.copy_(res)
-    ostore = _nan(((M + TAIL) * pitch + 16,), torch.bfloat16, cuda)
+    ostore = nan_buf(((M + TAIL) * pitch + 16,), torch.bfloat16, cuda)
     out = ostore[o_off:o_off + M * pitch].view(M, pitch)[:, :N]
     want = _expected_plan(path, 2 * o_off, 2 * r_off, 4 * b_off, pitch)
     args = dict(bias=bias, residual=resid, out=out, **kw)
@@ -869,12 +827,13 @@ def test_placement(cuda, path, operand, offset, parity):
     ops.gemm(a, wp, N, **args)
     torch.cuda.synchronize()
     y = ostore[o_off:o_off + (M + TAIL) * pitch].view(M + TAIL, pitch)
-    _layout_ok(y, M, N)
+    errs = layout(y, 0, N, "output", rows=M)
+    assert not errs, errs
     assert bool(torch.isnan(ostore[:o_off].float()).all()) and bool(torch.isnan(ostore[o_off + (M + TAIL) * pitch:].float()).all())
     acc = a.double() @ w.to(cuda).double().t()
     m = a.double().abs() @ w.to(cuda).double().abs().t()
     r, bound = gemm_expect(acc, m, K, bcol=bias.double(), res=res.double())
-    q = worst(y[:M, :N], r, bound)
+    q = max_ratio(y[:M, :N], r, bound)
     assert q <= 1.0, f"err/bound {q:.3g}"
 
 
@@ -887,13 +846,13 @@ def test_attention_out_placement(cuda, case):
     D = 512 if case.startswith("d512") else 64
     heads = 1 if D == 512 else 2
     B, nq, nkv, cols = 2, 100, 77, heads * D
-    g = _gen(51)
+    g = cpu_gen(51)
     q = (torch.randn((B, nq, cols), generator=g) * 2 ** 0.5).to(cuda).bfloat16()
     k = (torch.randn((B, nkv, cols), generator=g) * 2 ** 0.5).to(cuda).bfloat16()
     v = torch.randn((B, nkv, cols), generator=g).to(cuda).bfloat16()
     off = 1 if case.endswith("+1") else (2 if case.endswith("+2") else 0)
     bstride = nq * cols + (1 if "odd" in case else 0)
-    store = _nan((B * bstride + cols + 16,), torch.bfloat16, cuda)
+    store = nan_buf((B * bstride + cols + 16,), torch.bfloat16, cuda)
     out = store[off:].as_strided((B, nq, cols), (bstride, cols, 1))
     call = (lambda: ops.attention(q, k, v, heads, D ** -0.5, out=out)) if D == 64 else (lambda: ops.attention_d512(q, k, v, D ** -0.5, out=out))
     if off == 1 or "odd" in case:
@@ -908,5 +867,5 @@ def test_attention_out_placement(cuda, case):
     torch.cuda.synchronize()
     assert bool(torch.isnan(store[:off].float()).all())
     for b in range(B):
-        o, sv = _attn_ref(q[b].double(), k[b].double(), v[b].double(), heads, D, D ** -0.5)
-        assert worst(out[b], o, attn_expect(o, sv, nkv)) <= 1.0
+        o, sv = attn_ref(q[b].double(), k[b].double(), v[b].double(), heads, D, D ** -0.5)
+        assert max_ratio(out[b], o, attn_expect(o, sv, nkv)) <= 1.0

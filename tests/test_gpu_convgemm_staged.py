@@ -3,7 +3,7 @@
 A bf16 output whose rows are whole, 16-byte aligned chunks (c_out, out_pitch and residual_pitch multiples of 8) leaves the kernel
 through a shared-memory staging tile and 16-byte stores; any other output is stored from the accumulator fragment.  Each case here runs
 once with a NaN-padded output pitch that is a multiple of 8 (staged) and once with a pitch of c + 4 (fragment), on the same data:
-- the staged output is checked against float64 with the workload census's per-element bound, and its pitch gap must still be NaN;
+- the staged output is checked against float64 with the census's per-element bound (conv_expect), and its pitch gap must still be NaN;
 - the two outputs must be bitwise equal (same arithmetic, same order, one rounding to bf16).
 The cases cover every epilogue form, N tiles 32 / 64 / 128, M not a multiple of 128, c_out not a multiple of the N tile, convolution
 tiles spanning several rows and images (8x6 and 16x12 latents at batch 16) and the fused nearest-2x upsample."""
@@ -11,21 +11,17 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from test_gpu_workload_census import conv_expect, ratio
+from kernel_check import conv_expect, cpu_gen, max_ratio, nan_buf, same
 
 pytestmark = pytest.mark.gpu
 
 FORMS = ["bias", "nobias", "stepbias", "rowbias", "silu", "gelu", "relu", "geglu", "residual", "inplace", "rowscale", "silu_res_rowscale"]
 
 
-def _gen(seed):
-    return torch.Generator(device="cpu").manual_seed(seed)
-
-
 def _inputs(form, rows, c_out, c_eff, dev, seed):
     """Epilogue operands of one form: (ops kwargs, float64 column / row bias, residual bf16 [rows, c_eff] or None, row scale, act)."""
     from ladi_vton_b200 import ops
-    g = _gen(seed)
+    g = cpu_gen(seed)
     act = {"silu": ops.ACT_SILU, "gelu": ops.ACT_GELU, "relu": ops.ACT_RELU, "geglu": ops.ACT_GEGLU,
            "silu_res_rowscale": ops.ACT_SILU}.get(form, ops.ACT_NONE)
     kw, bcol, brow, res, rs = {"act": act}, None, None, None, None
@@ -51,24 +47,17 @@ def _inputs(form, rows, c_out, c_eff, dev, seed):
     return kw, bcol, brow, res, rs, act
 
 
-def _padded(rows, c, pitch, dev, fill=None):
-    t = torch.full((rows, pitch), float("nan"), dtype=torch.bfloat16, device=dev)
-    if fill is not None:
-        t[:, :c] = fill
-    return t
-
-
 def _run_both(call, form, rows, c_eff, res, dev):
     """call(out [rows, pitch] view, residual view or None, plan=False) for a staged pitch (c_eff + 8) and a fragment pitch (c_eff + 4);
     call(..., plan=True) returns the plan (ladi_conv2d_plan) of the same call, which must be the staged one and the fragment one."""
     outs = []
     for pitch, staged in ((c_eff + 8, 1), (c_eff + 4, 0)):
         if form == "inplace":
-            buf = _padded(rows, c_eff, pitch, dev, res)
+            buf = nan_buf((rows, pitch), torch.bfloat16, dev, res)
             rbuf = buf[:, :c_eff]
         else:
-            buf = _padded(rows, c_eff, pitch, dev)
-            rbuf = None if res is None else _padded(rows, c_eff, pitch, dev, res)[:, :c_eff]
+            buf = nan_buf((rows, pitch), torch.bfloat16, dev)
+            rbuf = None if res is None else nan_buf((rows, pitch), torch.bfloat16, dev, res)[:, :c_eff]
         plan = call(buf, rbuf, plan=True)
         assert (plan.staged, plan.splits, plan.pair) == (staged, 1, 0), f"pitch {pitch}: staged {plan.staged}, want {staged}"
         call(buf, rbuf)
@@ -77,7 +66,7 @@ def _run_both(call, form, rows, c_eff, res, dev):
     staged, frag = outs
     assert bool(torch.isnan(staged[:, c_eff:].float()).all()), "the staged drain wrote into the pitch gap"
     assert bool(torch.isfinite(staged[:, :c_eff].float()).all()), "the staged drain left output elements unwritten"
-    assert torch.equal(staged[:, :c_eff].view(torch.int16), frag[:, :c_eff].view(torch.int16)), "staged and fragment stores differ"
+    assert same(staged[:, :c_eff], frag[:, :c_eff]), "staged and fragment stores differ"
     return staged[:, :c_eff]
 
 
@@ -94,7 +83,7 @@ def _check(y, acc, m, K, bcol, brow, res, rs, act):
         r64 = res.double()
         mm += r64.abs()
     r, bound = conv_expect(pre, mm, K, act, r64, None if rs is None else rs[:, None])
-    worst = float(ratio(y, r, bound).max())
+    worst = max_ratio(y, r, bound)
     assert worst <= 1.0, f"err/bound {worst:.3g}"
 
 
@@ -106,7 +95,7 @@ def test_staged_gemm(cuda, form, bn):
     M, K = 1000, 320
     c_out = 640 if form == "geglu" else 320
     c_eff = c_out // 2 if form == "geglu" else c_out
-    g = _gen(11)
+    g = cpu_gen(11)
     a = torch.randn((M, K), generator=g).to(cuda).bfloat16()
     w = (torch.randn((c_out, K), generator=g) * K ** -0.5).to(cuda).bfloat16()
     kw, bcol, brow, res, rs, act = _inputs(form, M, c_out, c_eff, cuda, 12)
@@ -135,7 +124,7 @@ def test_staged_conv(cuda, form, shape):
     h, w = (8, 6) if shape.endswith("8x6") else (16, 12)
     ho, wo = (2 * h, 2 * w) if up else (h, w)
     rows = n * ho * wo
-    g = _gen(21)
+    g = cpu_gen(21)
     x = torch.randn((n, h, w, C), generator=g).to(cuda).bfloat16()
     wt = (torch.randint(-7, 8, (c_out, C, 3, 3), generator=g).float() / 64).to(cuda)
     kw, bcol, brow, res, rs, act = _inputs(form, rows, c_out, c_out, cuda, 22)

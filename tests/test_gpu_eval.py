@@ -16,13 +16,11 @@ import numpy as np
 import pytest
 import torch
 
+from kernel_check import rel_l2
+from model_pairs import CTX, NV, cli_models
+
 pytestmark = pytest.mark.gpu
 EIN, EOUT = [128, 128, 128, 256, 512], [128, 256, 512, 512, 512]
-
-
-def rel_l2(y, ref):
-    y, ref = y.detach().float().cpu(), ref.detach().float().cpu()
-    return ((y - ref).norm() / ref.norm().clamp_min(1e-12)).item()
 
 
 @pytest.mark.parametrize("kw", [dict(type="linear", padding=1), dict(kernel_size=1, padding=0)], ids=["linear", "k1"])
@@ -86,19 +84,17 @@ def test_inversion_adapter_two_layers_full(cuda):
 
 
 # ---- the generate_images_from_tryon_pipe body with reduced-width models -------------------------------------------------------------
-NV = 4
 
 
 @pytest.fixture(scope="module")
 def models(cuda):
-    """test_gpu_cli's engine / oracle pairs (same seeded weights), plus a 27-channel UNet, linear and 1x1 EMASC and a 2-layer adapter."""
-    from test_gpu_cli import CTX, _models
+    """The CLI tests' engine / oracle pairs (model_pairs.cli_models, same seeded weights), plus a 27-channel UNet, linear and 1x1 EMASC and a 2-layer adapter."""
     from ladi_oracle.emasc_forms import EMASC as OE
     from ladi_oracle.parts import InversionAdapter as OA
     from ladi_oracle.unet import UNet2DConditionModel as OU
     from ladi_vton_b200 import EMASC, InversionAdapter, UNet2DConditionModel, synthetic as S
     from ladi_vton_b200.unet import unet_param_shapes
-    eng, orc = _models(cuda)
+    eng, orc = cli_models(cuda)
     ein, eout = S.emasc_channels(S.SMALL_VAE["block_out_channels"])
     for name, kw, seed in (("linear", dict(type="linear", padding=1), 61), ("k1", dict(kernel_size=1, padding=0), 62)):
         e = EMASC(ein, eout, **kw)

@@ -6,12 +6,10 @@ bit-exactly against the same bf16 arithmetic in torch; attention <= 1e-2; whole 
 import pytest
 import torch
 
+from kernel_check import rel_l2
+from model_pairs import text_pair
+
 pytestmark = pytest.mark.gpu
-
-
-def rel_l2(y, ref):
-    y, ref = y.detach().float().cpu(), ref.detach().float().cpu()
-    return ((y - ref).norm() / ref.norm().clamp_min(1e-12)).item()
 
 
 @pytest.mark.parametrize("B,heads,hd,nq,causal", [(2, 16, 80, 257, False), (3, 16, 64, 77, True), (1, 2, 8, 5, True), (2, 3, 128, 130, False),
@@ -65,21 +63,6 @@ def test_embed_patchify_assemble_exact(cuda):
     assert torch.equal(x, ref)
 
 
-def _text_pair(cuda, seed, **cfg):
-    from ladi_vton_b200 import CLIPTextModel, synthetic as S
-    from ladi_oracle.clip import ClipTextEncoder
-    eng = CLIPTextModel(**cfg)
-    c = eng.config
-    sd = S.random_state_dict(eng.param_shapes(), seed)
-    for k in sd:  # unit-variance embeddings (library init scale is irrelevant behind the first LayerNorm, but keep the sum meaningful)
-        if "embedding" in k:
-            sd[k] = torch.randn(sd[k].shape, generator=torch.Generator().manual_seed(seed + len(k)))
-    o = ClipTextEncoder(vocab=c.vocab_size, dim=c.hidden_size, heads=c.num_attention_heads, layers=c.num_hidden_layers,
-                        mlp=c.intermediate_size, max_pos=c.max_position_embeddings).eval()
-    o.load_state_dict(sd)
-    return eng.load_state_dict(sd).to(cuda), o
-
-
 def _ids(B, T, vocab, g, dollars=()):
     ids = torch.randint(1, min(vocab, 250), (B, T), generator=g)
     ids[:, 0] = vocab - 2
@@ -96,7 +79,7 @@ def test_encode_text_word_embedding(cuda, full):
     from ladi_vton_b200 import encode_text_word_embedding
     from ladi_oracle.clip import encode_text_word_embedding as oracle_fn
     cfg = {} if full else dict(vocab_size=1000, hidden_size=128, intermediate_size=512, num_hidden_layers=3, num_attention_heads=2)
-    eng, o = _text_pair(cuda, 77, **cfg)
+    eng, o = text_pair(cuda, 77, **cfg)
     g = torch.Generator().manual_seed(11)
     nv = 16 if full else 4
     ids = _ids(3, 77, eng.config.vocab_size, g, dollars=[(0, 5, nv), (2, 8, nv)])
@@ -119,7 +102,7 @@ def test_encode_text_word_embedding(cuda, full):
 
 def test_text_encoder_errors(cuda):
     from ladi_vton_b200 import CLIPTextModel, encode_text_word_embedding
-    eng, _ = _text_pair(cuda, 5, vocab_size=1000, hidden_size=64, intermediate_size=128, num_hidden_layers=1, num_attention_heads=1)
+    eng, _ = text_pair(cuda, 5, vocab_size=1000, hidden_size=64, intermediate_size=128, num_hidden_layers=1, num_attention_heads=1)
     ids = torch.randint(1, 200, (2, 77))
     ids[0, 75] = 259
     with pytest.raises(IndexError):
@@ -161,7 +144,7 @@ def test_pipeline_with_native_text_encoder(cuda):
     tokenizer + text_encoder; the engine text tower plugs into that slot."""
     from ladi_vton_b200 import synthetic as S
     pipe, _ = S.build_pipeline(cuda, S.SMALL_UNET, S.SMALL_VAE)
-    eng, _ = _text_pair(cuda, 8, vocab_size=1000, hidden_size=128, intermediate_size=256, num_hidden_layers=2, num_attention_heads=2)
+    eng, _ = text_pair(cuda, 8, vocab_size=1000, hidden_size=128, intermediate_size=256, num_hidden_layers=2, num_attention_heads=2)
 
     class Tok:
         model_max_length = 77

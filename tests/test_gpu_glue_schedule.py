@@ -1,7 +1,7 @@
 """The glue, cloth-warping and front-end kernels (csrc/warp.cu, the non-norm half of csrc/pointwise.cu, csrc/frontend.cu's small kernels)
 at the edges of their launch policy and of their value ranges, against float64, and the placement rules of their entry points.
 
-Shapes and values no workload reaches are driven through the glue census's own replays (tests/test_gpu_glue_frontend_census.py):
+Shapes and values no workload reaches are driven through the glue census's replays (tests/kernel_check.py):
 synthetic descriptors in the field names of its SCHEMA, so every case gets the census's float64 reference and per-element bound, its
 NaN-poisoned outputs with a tail, its column-window checks and its second, bit-identical run.  The descriptors are not census rows: the
 census records what the workloads run.
@@ -30,20 +30,15 @@ References added here (the census has none for these entry points):
 CPU tests at the end show the new references have teeth (an fp32 emulation passes; x / y swapped, a nearest index off by one, floorf in
 place of rintf and a NaN-dropping clamp or max are rejected), and check every placement rule in a process that sees no device."""
 import ctypes as C
-import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
-from test_gpu_glue_frontend_census import NAN, REPLAY, SCHEMA, _buf, _determinism, _exact, _tail_nan, _twice, _worst
-from test_gpu_workload_census import EPS24, Replay, ratio
+from kernel_check import (A, EPS24, NAN, REPLAY, SCHEMA, SMS, Replay, check_placement, determinism, exact, flat_buf, ratio, sms, tail_nan, twice,
+                          worst_at)
 
-SMS_CPU = 132  # the H100 SXM's SM count: what the CPU tests assume for the cases' shapes
 PASS = 16 * 256  # elements per SM in one full grid-stride pass
 INF = float("inf")
 
@@ -108,12 +103,12 @@ def replay_nhwc_to_nchw_f32(R, f):
     cnt = n * c * h * w
 
     def fresh():
-        flat, o = _buf(R, cnt, torch.float32)
+        flat, o = flat_buf(R, cnt, torch.float32)
         return dict(flat=flat, out=o)
-    runs = _twice(lambda b: lib.call("ladi_nhwc_to_nchw_f32", C.c_void_p(x.data_ptr()), f32, n, c, h, w, xp, c_off, C.c_void_p(b["out"].data_ptr()),
+    runs = twice(lambda b: lib.call("ladi_nhwc_to_nchw_f32", C.c_void_p(x.data_ptr()), f32, n, c, h, w, xp, c_off, C.c_void_p(b["out"].data_ptr()),
                                      R.stream), fresh)
-    errs = _tail_nan(runs[0]["flat"], cnt, "output") + _determinism(runs, ["flat"])
-    e, res = _exact(runs[0]["out"].view(n, c, h, w), nhwc_to_nchw_expect(x, n, h, w, c, c_off), "values")
+    errs = tail_nan(runs[0]["flat"], cnt, "output") + determinism(runs, ["flat"])
+    e, res = exact(runs[0]["out"].view(n, c, h, w), nhwc_to_nchw_expect(x, n, h, w, c, c_off), "values")
     return errs + e, res
 
 
@@ -124,11 +119,11 @@ def replay_upsample2x_nhwc(R, f):
     cnt = n * 4 * h * w * c
 
     def fresh():
-        flat, o = _buf(R, cnt, torch.bfloat16)
+        flat, o = flat_buf(R, cnt, torch.bfloat16)
         return dict(flat=flat, out=o)
-    runs = _twice(lambda b: lib.call("ladi_upsample2x_nhwc", C.c_void_p(x.data_ptr()), n, h, w, c, C.c_void_p(b["out"].data_ptr()), R.stream), fresh)
-    errs = _tail_nan(runs[0]["flat"], cnt, "output") + _determinism(runs, ["flat"])
-    e, res = _exact(runs[0]["out"].view(n, 2 * h, 2 * w, c), upsample_nearest_expect(x), "values")
+    runs = twice(lambda b: lib.call("ladi_upsample2x_nhwc", C.c_void_p(x.data_ptr()), n, h, w, c, C.c_void_p(b["out"].data_ptr()), R.stream), fresh)
+    errs = tail_nan(runs[0]["flat"], cnt, "output") + determinism(runs, ["flat"])
+    e, res = exact(runs[0]["out"].view(n, 2 * h, 2 * w, c), upsample_nearest_expect(x), "values")
     return errs + e, res
 
 
@@ -146,13 +141,13 @@ def replay_pose_heatmaps(R, f, kpts=None):
     cnt = m * h * w
 
     def fresh():
-        flat, o = _buf(R, cnt, torch.float32)
+        flat, o = flat_buf(R, cnt, torch.float32)
         return dict(flat=flat, out=o)
-    runs = _twice(lambda b: lib.call("ladi_pose_heatmaps", C.c_void_p(k.data_ptr()), m, h, w, float(sigma), C.c_void_p(b["out"].data_ptr()),
+    runs = twice(lambda b: lib.call("ladi_pose_heatmaps", C.c_void_p(k.data_ptr()), m, h, w, float(sigma), C.c_void_p(b["out"].data_ptr()),
                                      R.stream), fresh)
-    errs = _tail_nan(runs[0]["flat"], cnt, "output") + _determinism(runs, ["flat"])
+    errs = tail_nan(runs[0]["flat"], cnt, "output") + determinism(runs, ["flat"])
     r, bound = pose_expect(k.double(), h, w, float(np.float32(sigma)))
-    e, res = _worst(ratio(runs[0]["out"].view(m, h, w), r, bound), ("map", "y", "x"))
+    e, res = worst_at(ratio(runs[0]["out"].view(m, h, w), r, bound), ("map", "y", "x"))
     return errs + e, res
 
 
@@ -161,10 +156,10 @@ def replay_check_binarise_values(R, f, image_values, mask_values, flags0):
     flags0 OR the reference's range tests (NaN compares false), the mask binarised at 0.5 with NaN kept."""
     from ladi_vton_b200 import lib
     ni, nm = f["n_image"], f["n_mask"]
-    image_flat, image = _buf(R, ni, torch.float32, fill=5.0)
+    image_flat, image = flat_buf(R, ni, torch.float32, fill=5.0)
     image.copy_(R.rand(ni) * 2 - 1)
     image[:len(image_values)] = torch.tensor(image_values, dtype=torch.float32)
-    mflat, m = _buf(R, nm, torch.float32, fill=0.3)
+    mflat, m = flat_buf(R, nm, torch.float32, fill=0.3)
     m.copy_(R.rand(nm))
     m[nm - len(mask_values):] = torch.tensor(mask_values, dtype=torch.float32)  # at the end: the last elements of the grid-stride walk
     src = m.clone()
@@ -176,7 +171,7 @@ def replay_check_binarise_values(R, f, image_values, mask_values, flags0):
     errs = [] if flags.tolist() == want else [f"flags {flags.tolist()}, expected {want}"]
     if not bool((mflat[nm:] == 0.3).all()):
         errs.append("mask written past n_mask")
-    errs += _exact(m, torch.where(src < 0.5, 0.0, torch.where(src >= 0.5, 1.0, src)), "mask")[0]
+    errs += exact(m, torch.where(src < 0.5, 0.0, torch.where(src >= 0.5, 1.0, src)), "mask")[0]
     return errs, (0.0 if not errs else INF, "bit-exact mask and flags" if not errs else errs[0])
 
 
@@ -418,8 +413,8 @@ def _work(kind, f):
 # ================================================================================================================ CPU: the cases
 def test_edge_cases_are_what_they_say():
     """The cases hit the limits they are named after, at the H100 SXM's 132 SMs (CPU)."""
-    E = {name: (kind, f) for name, kind, f, _ in edges(SMS_CPU)}
-    P = PASS * SMS_CPU
+    E = {name: (kind, f) for name, kind, f, _ in edges(SMS)}
+    P = PASS * SMS
     for name, (kind, f) in E.items():
         if "full pass" in name:
             assert _work(kind, f) == P, name
@@ -449,11 +444,11 @@ def test_teeth_nhwc_to_nchw_xy_swap():
     x = torch.randn(n * h * w, xp, generator=g)
     r = nhwc_to_nchw_expect(x, n, h, w, c, co)
     good = x.view(n, h, w, xp)[..., co:co + c].permute(0, 3, 1, 2)
-    assert not _exact(good, r, "")[0]
+    assert not exact(good, r, "")[0]
     swapped = x.view(n, w, h, xp)[..., co:co + c].permute(0, 3, 2, 1)  # x / y swapped in the source index
-    assert _exact(swapped.contiguous(), r, "")[0]
+    assert exact(swapped.contiguous(), r, "")[0]
     shifted = x.view(n, h, w, xp)[..., co - 1:co - 1 + c].permute(0, 3, 1, 2)  # c_off ignored by one
-    assert _exact(shifted.contiguous(), r, "")[0]
+    assert exact(shifted.contiguous(), r, "")[0]
 
 
 def test_teeth_upsample_nearest_off_by_one():
@@ -462,9 +457,9 @@ def test_teeth_upsample_nearest_off_by_one():
     r = upsample_nearest_expect(x)
     oy, ox = torch.arange(8), torch.arange(6)
     good = x[:, oy // 2][:, :, ox // 2]
-    assert not _exact(good.contiguous(), r, "")[0]
+    assert not exact(good.contiguous(), r, "")[0]
     bad = x[:, ((oy + 1) // 2).clamp_max(3)][:, :, ox // 2]
-    assert _exact(bad.contiguous(), r, "")[0]
+    assert exact(bad.contiguous(), r, "")[0]
 
 
 def _pose_emulate(k, h, w, sigma, rnd=torch.round):
@@ -493,21 +488,20 @@ def test_teeth_nan_dropping_clamp_and_max():
     x = torch.tensor([NAN, -2.0, 0.5, INF, -INF, 2.0, NAN, 0.0])
     ref = x.clamp(-1.0, 1.0)
     keep = torch.where(torch.isnan(x), x, torch.fmin(torch.fmax(x, torch.tensor(-1.0)), torch.tensor(1.0)))
-    assert not _exact(keep, ref, "")[0]
+    assert not exact(keep, ref, "")[0]
     drop = torch.fmin(torch.fmax(x, torch.tensor(-1.0)), torch.tensor(1.0))  # fmaxf / fminf: NaN -> the other operand
-    assert _exact(drop, ref, "")[0]
+    assert exact(drop, ref, "")[0]
     X = torch.randn(1, 8, 4, 6).bfloat16()
     X[0, 3, 1, 2] = NAN
     ref = F.max_pool2d(X.float(), 2).bfloat16()
     win = X.float().unfold(2, 2, 2).unfold(3, 2, 2).reshape(1, 8, 2, 3, 4)
     keep = win.amax(-1).bfloat16()  # NaN-propagating
-    assert not _exact(keep, ref, "")[0]
+    assert not exact(keep, ref, "")[0]
     drop = torch.nan_to_num(win, nan=-INF).amax(-1).bfloat16()
-    assert _exact(drop, ref, "")[0]
+    assert exact(drop, ref, "")[0]
 
 
 # ================================================================================================================ CPU: placement rules
-A = 1 << 20  # a fake, 256-byte aligned device address; never dereferenced
 # (id, entry point, arguments with pointers as ints, expected message or None = the checks pass and the launch fails for lack of a device)
 _ADD = lambda a=A, b=A, out=A: ("ladi_add_bf16", [a, b, out, 64])  # noqa: E731
 _UP = lambda x=A, out=A: ("ladi_upsample2x_nhwc", [x, 1, 2, 2, 8, out])  # noqa: E731
@@ -584,56 +578,28 @@ PLACEMENT = [
     ("bilinear_down8 null out", "ladi_bilinear_down8", [A, 1, 1, 8, 8, 0], "bilinear_down8: null operand"),
     ("bilinear_down8 ok", "ladi_bilinear_down8", [A, 1, 1, 8, 8, A], None),
 ]
-_CHILD = r"""
-import ctypes as C, json, sys
-sys.path.insert(0, sys.argv[1])
-from ladi_vton_b200 import lib
-L = lib.load()
-res = []
-for name, args in json.loads(sys.argv[2]):
-    fn = getattr(L, name)
-    rc = fn(*[C.c_void_p(a) if t is C.c_void_p else a for a, t in zip(args, fn.argtypes)], None)
-    res.append([rc, L.ladi_last_error().decode()])
-print(json.dumps(res))
-"""
 
 
 def test_placement_rules_without_a_device():
-    """Each rule rejects with LADI_ERR_INVALID and a message naming the operand; a placement that meets the rules passes the checks and
-    then fails with LADI_ERR_CUDA, because the child process sees no device: no call here can launch a kernel."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
-    out = subprocess.run([sys.executable, "-c", _CHILD, root, json.dumps([[n, a] for _, n, a, _ in PLACEMENT])], env=env, capture_output=True,
-                         text=True, timeout=120)
-    assert out.returncode == 0, out.stderr
-    res = json.loads(out.stdout.strip().splitlines()[-1])
-    bad = []
-    for (what, name, _, want), (rc, msg) in zip(PLACEMENT, res):
-        if want is None:
-            if rc != 2:
-                bad.append(f"{what}: rc {rc} ({msg}); expected the checks to pass and the launch to fail without a device")
-        elif rc != 1 or want not in msg:
-            bad.append(f"{what}: rc {rc} ({msg}); expected LADI_ERR_INVALID with '{want}'")
-    assert not bad, "\n".join(bad)
+    """The placement rules of the glue, warping and front-end entry points (PLACEMENT), checked in a process that sees no device."""
+    check_placement(PLACEMENT)
 
 
 # ================================================================================================================ GPU
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-_EDGE_IDS = [e[0] for e in edges(SMS_CPU)]
+_EDGE_IDS = [e[0] for e in edges(SMS)]
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", _EDGE_IDS)
 def test_glue_edge_against_float64(cuda, name):
-    case = {e[0]: e for e in edges(_sms())}[name]
+    case = {e[0]: e for e in edges(sms(cuda))}[name]
     _, kind, f, kw = case
     R = Replay(cuda, 1357)
     kw = {k: (v(R, f) if callable(v) else v) for k, v in kw.items()}
     errs, res = REPLAY_HERE[kind](R, f, **kw)
-    print(f"\n{name} at {_sms()} SMs: err/bound {res[0]:.3g} ({res[1]})")
+    print(f"\n{name} at {sms(cuda)} SMs: err/bound {res[0]:.3g} ({res[1]})")
     torch.cuda.empty_cache()
     assert not errs, f"{name}:\n  " + "\n  ".join(errs)
 

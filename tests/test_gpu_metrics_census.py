@@ -6,13 +6,13 @@ with the ABI calls recorded instead of launched (`lib.RECORD`): `FIDInceptionV3.
 resize of 512x384 images to 299x299, then the Inception), `LPIPSAlex.__call__` on B pairs (2B images through AlexNet) and `metrics.ssim`
 at 512x384.  Batches: 32 (`compute_metrics`' default), 64 (`bench_metrics.py`), 1, and the ragged last batches at batch 32 of the
 standard test splits (VITON-HD's 2032 pairs leave 16, a Dress Code category's 1800 leave 8).  Convolutions / GEMMs go through
-test_engine_trace.python_trace in the workload census's fields (those either other census replays are skipped); their plans are queried
+python_trace in the workload census's fields (those either other census replays are skipped); their plans are queried
 with the production split-K workspace (ops.SPLITK_WS_BYTES), because under `lib.RECORD` `ops.splitk_workspace` hands out a 4 KB stub
 that would rule split-K out.  Every other entry point needs a row in this file's SCHEMA, or test_metrics_census_integrity fails.
 Every recorded GEMM output starts at a multiple of 8 columns of its concatenation (asserted), so replaying it at column 0 of a
 buffer of the same pitch takes the same plan.
 
-The replay (GPU).  Conv / GEMM through the workload census's replay_conv.  Every other kind on fresh buffers: NaN input pitch gaps, a
+The replay (GPU).  Conv / GEMM through the workload census's replay_conv (tests/kernel_check.py).  Every other kind on fresh buffers: NaN input pitch gaps, a
 NaN-poisoned output with a tail, the call's columns finite afterwards and everything else NaN (a pool into a concatenation slice leaves
 the other channels NaN; `lpips_layer` adds to a non-zero `acc` and touches nothing else), and a second run bit-identical.
 
@@ -47,25 +47,18 @@ Placement rules of the metrics entry points are tested on the CPU in a child pro
 return the named error; a call that passes its checks fails for lack of a device instead, so these tests never launch a kernel."""
 import ctypes as C
 import functools
-import json
 import math
-import os
-import subprocess
-import sys
 import time
-from collections import OrderedDict, defaultdict
+from collections import defaultdict
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-from test_gpu_glue_frontend_census import (_buf, _cpu_pack, _determinism, _exact, _record, _tail_nan, _twice, _window, _worst,
-                                           assert_all_known, describe, glue_census)
-from test_gpu_workload_census import Replay, census, parse, ratio, replay_conv
+from kernel_check import (A, EPS24, ROUND1, SMS, Replay, assert_all_known, census, check_library_defaults, check_placement, collect, cpu_pack,
+                          describe, determinism, exact, flat_buf, glue_census, key_of, layout, max_ratio, parse, pick, ptr, python_trace, ratio,
+                          recorded, replay_conv, tail_nan, twice, worst_at)
 
-EPS24 = 2.0 ** -24
-ROUND1 = 2.0 ** -8
-SMS = 132
 POOL_MAX, POOL_AVG, POOL_EXCL, POOL_GLOBAL = 0, 1, 2, 3
 SSIM_C1, SSIM_C2 = 0.01 ** 2, 0.03 ** 2
 
@@ -88,7 +81,7 @@ BATCHES = [("batch 32 (compute_metrics default)", 32), ("batch 64 (tools/bench_m
 def _nets():
     from ladi_vton_b200.metrics import FIDInceptionV3, LPIPSAlex, random_state_dict
     inc, lp = FIDInceptionV3(), LPIPSAlex()
-    return _cpu_pack(inc, random_state_dict(inc.param_shapes(), 0)), _cpu_pack(lp, random_state_dict(lp.param_shapes(), 1))
+    return cpu_pack(inc, random_state_dict(inc.param_shapes(), 0)), cpu_pack(lp, random_state_dict(lp.param_shapes(), 1))
 
 
 def _metrics_calls(B, H=512, W=384):
@@ -100,11 +93,7 @@ def _metrics_calls(B, H=512, W=384):
         inc.is_features(torch.zeros((B, 3, H, W)))  # IS: TF1 resize, then the same network
         lp(torch.zeros((B, 3, H, W)), torch.zeros((B, 3, H, W)))
         M.ssim(torch.zeros((B, 3, H, W)), torch.zeros((B, 3, H, W)))
-    return _record(run)
-
-
-def _key(kind, f):
-    return kind + " " + " ".join(f"{k}={v}" for k, v in f.items())
+    return recorded(run)
 
 
 def conv_plan_at_production_ws(desc):
@@ -115,48 +104,37 @@ def conv_plan_at_production_ws(desc):
     return lib.conv_plan(q, SMS)
 
 
-def collect(work):
+def metrics_collect(work):
     """work = [(label, () -> recorded calls)] -> (desc, calls, unknown, misplaced): desc = OrderedDict key -> {kind, f, first, n, plan}
     of the descriptors neither other census replays; calls = {label: {kind: [calls, set of keys]}}; unknown = entry points recorded
     without a SCHEMA row; misplaced = GEMM outputs that do not start at a multiple of 8 columns."""
-    import test_engine_trace as tt
     known = set(census()[0]) | {k for k, d in glue_census()[0].items() if d["kind"] == "conv"}
-    desc, calls, unknown, misplaced = OrderedDict(), OrderedDict(), [], []
-    for wl, rec in work:
-        cnt = calls.setdefault(wl, defaultdict(lambda: [0, set()]))
-        for name, args in rec():
-            plan = None
-            if name == "ladi_conv2d_bf16":
-                d = args[0]._obj
-                if d.out % 16:  # bf16 columns: the CPU allocator's blocks are 64-byte aligned, so this is the column offset mod 8
-                    misplaced.append(f"out column offset {d.out % 16 // 2} mod 8")
-                op, f = parse(tt.python_trace([(name, args)])[0])
-                kind, key = op, _key(op, f)
-                f = {k: int(v) for k, v in f.items()}
-                if key in known:
-                    cnt[kind][0] += 1
-                    continue
-                plan = conv_plan_at_production_ws(d)
-                plan = dict(bn=plan.bn, splits=plan.splits, staged=plan.staged)
-            elif name in SCHEMA:
-                kind, f = describe(name, args, SCHEMA)
-                key = _key(kind, f)
-            else:
-                unknown.append(name)
-                continue
-            cnt[kind][0] += 1
-            cnt[kind][1].add(key)
-            if key not in desc:
-                desc[key] = dict(kind=kind, f=f, first=wl, n=0, plan=plan)
-            desc[key]["n"] += 1
+    unknown, misplaced = [], []
+
+    def classify(call):
+        name, args = call
+        if name == "ladi_conv2d_bf16":
+            d = args[0]._obj
+            if d.out % 16:  # bf16 columns: the CPU allocator's blocks are 64-byte aligned, so this is the column offset mod 8
+                misplaced.append(f"out column offset {d.out % 16 // 2} mod 8")
+            op, f = parse(python_trace([call])[0])
+            if key_of(op, f) in known:
+                return op, key_of(op, f), None, None
+            plan = conv_plan_at_production_ws(d)
+            return op, key_of(op, f), {k: int(v) for k, v in f.items()}, dict(plan=dict(bn=plan.bn, splits=plan.splits, staged=plan.staged))
+        if name in SCHEMA:
+            kind, f = describe(name, args, SCHEMA)
+            return kind, key_of(kind, f), f, dict(plan=None)
+        unknown.append(name)
+        return None
+    desc, calls = collect([(wl, wl, rec) for wl, rec in work], classify)
     return desc, calls, unknown, misplaced
 
 
 @functools.lru_cache(maxsize=None)
 def metrics_census():
-    for k in ("LADI_UP2X", "LADI_LN_FOLD", "LADI_CONV_2CTA"):
-        assert k not in os.environ, f"census runs with library defaults; unset {k}"
-    return collect([(wl, functools.partial(_metrics_calls, B)) for wl, B in BATCHES])
+    check_library_defaults()
+    return metrics_collect([(wl, functools.partial(_metrics_calls, B)) for wl, B in BATCHES])
 
 
 # ================================================================================================================ references and bounds
@@ -286,8 +264,6 @@ def resize_expect(x, oh, ow):
 
 
 # ================================================================================================================ replay (GPU)
-def _P(t):
-    return C.c_void_p(t.data_ptr() if t is not None else 0)
 
 
 def _features(R, rows, c):
@@ -318,30 +294,26 @@ def replay_im2col(R, f):
         x, shift, scale = R.poisoned(n * h * w, pitch, _features(R, n * h * w, c)), None, None
 
     def fresh():
-        flat, o = _buf(R, rows * kp, torch.bfloat16)
+        flat, o = flat_buf(R, rows * kp, torch.bfloat16)
         return dict(flat=flat, out=o)
-    runs = _twice(lambda b: lib.call("ladi_im2col_bf16", _P(x), f["f32"], n, c, h, w, pitch, kh, kw, sh, sw, ph, pw, _P(shift), _P(scale),
-                                     _P(b["out"]), kp, R.stream), fresh)
+    runs = twice(lambda b: lib.call("ladi_im2col_bf16", ptr(x), f["f32"], n, c, h, w, pitch, kh, kw, sh, sw, ph, pw, ptr(shift), ptr(scale),
+                                     ptr(b["out"]), kp, R.stream), fresh)
     out = runs[0]["out"].view(n, oh * ow, kp)
-    errs = _window(out.view(rows, kp), 0, kp, "rows") + _tail_nan(runs[0]["flat"], rows * kp, "rows") + _determinism(runs, ["flat"])
+    errs = layout(out.view(rows, kp), 0, kp, "rows") + tail_nan(runs[0]["flat"], rows * kp, "rows") + determinism(runs, ["flat"])
     worst = (0.0, "bit-exact")
-    for b in _pick_images(n, rows * kp):
+    for b in pick(n, rows * kp, 1 << 28):
         y = out[b]
         if f["f32"]:
             q = ((x[b:b + 1] - shift.view(-1, 1, 1)) / scale.view(-1, 1, 1)).bfloat16()  # torch fp32, IEEE division
-            e, _ = _exact(y, im2col_ref(q.permute(0, 2, 3, 1), *geo), f"image {b}: against bf16 of torch's fp32 affine")
+            e, _ = exact(y, im2col_ref(q.permute(0, 2, 3, 1), *geo), f"image {b}: against bf16 of torch's fp32 affine")
             r, bound = im2col_pixel_expect(x[b:b + 1], shift, scale, geo)
-            e2, res = _worst(ratio(y, r, bound), ("row", "column"), f" of image {b}")
+            e2, res = worst_at(ratio(y, r, bound), ("row", "column"), f" of image {b}")
             errs += e + e2
             worst = max(worst, res)
         else:
-            e, _ = _exact(y, im2col_ref(x.view(n, h, w, pitch)[b:b + 1, ..., :c], *geo), f"image {b}")
+            e, _ = exact(y, im2col_ref(x.view(n, h, w, pitch)[b:b + 1, ..., :c], *geo), f"image {b}")
             errs += e
     return errs, worst
-
-
-def _pick_images(n, work, limit=1 << 28):
-    return list(range(n)) if n <= 2 or work <= limit else [0, n - 1]
 
 
 def replay_pool2d(R, f, values=None):
@@ -358,22 +330,22 @@ def replay_pool2d(R, f, values=None):
     rows = n * oh * ow
 
     def fresh():
-        flat, o = _buf(R, rows * op, dt)
+        flat, o = flat_buf(R, rows * op, dt)
         return dict(flat=flat, out=o)
-    runs = _twice(lambda b: lib.call("ladi_pool2d_bf16", _P(x), n, h, w, c, xp, k, s, p, mode, _P(b["out"]), op, c_off, R.stream), fresh)
+    runs = twice(lambda b: lib.call("ladi_pool2d_bf16", ptr(x), n, h, w, c, xp, k, s, p, mode, ptr(b["out"]), op, c_off, R.stream), fresh)
     out = runs[0]["out"].view(rows, op)
-    errs = _window(out, c_off, c_off + c, "output") + _tail_nan(runs[0]["flat"], rows * op, "output") + _determinism(runs, ["flat"])
+    errs = layout(out, c_off, c_off + c, "output") + tail_nan(runs[0]["flat"], rows * op, "output") + determinism(runs, ["flat"])
     y = out[:, c_off:c_off + c]
     if mode == POOL_GLOBAL:
         r, bound = global_avg_expect(X)
-        e, res = _worst(ratio(y, r, bound), ("image", "channel"))
+        e, res = worst_at(ratio(y, r, bound), ("image", "channel"))
         return errs + e, res
     r, bound = pool_expect(X, k, s, p, mode)
     r, bound = (t.permute(0, 2, 3, 1).reshape(rows, c) for t in (r, bound))
     if mode == POOL_MAX:
-        e, res = _exact(y.contiguous(), r.bfloat16(), "max pool")
+        e, res = exact(y.contiguous(), r.bfloat16(), "max pool")
         return errs + e, res
-    e, res = _worst(ratio(y, r, bound), ("output pixel", "channel"))
+    e, res = worst_at(ratio(y, r, bound), ("output pixel", "channel"))
     return errs + e, res
 
 
@@ -392,23 +364,23 @@ def replay_lpips_layer(R, f, self_pair=False, calls=1):
     hw = h * w
     feats = R.poisoned(2 * n * hw, pitch, _lpips_features(R, n, hw, c))
     fa, fb = feats[:n * hw], (feats[:n * hw] if self_pair else feats[n * hw:])
-    lin_flat, lin = _buf(R, c, torch.float32)
+    lin_flat, lin = flat_buf(R, c, torch.float32)
     lin.copy_(R.rand(c) * 0.1)
     acc0 = R.rand(n) + 0.25
 
     def fresh():
-        flat, a = _buf(R, n, torch.float32)
+        flat, a = flat_buf(R, n, torch.float32)
         a.copy_(acc0)
         return dict(flat=flat, acc=a)
 
     def call(b):
         for _ in range(calls):
-            lib.call("ladi_lpips_layer", _P(fa), _P(fb), n, h, w, c, pitch, _P(lin), _P(b["acc"]), R.stream)
-    runs = _twice(call, fresh)
+            lib.call("ladi_lpips_layer", ptr(fa), ptr(fb), n, h, w, c, pitch, ptr(lin), ptr(b["acc"]), R.stream)
+    runs = twice(call, fresh)
     acc = runs[0]["acc"]
-    errs = _tail_nan(runs[0]["flat"], n, "acc") + _tail_nan(lin_flat, c, "lin") + _determinism(runs, ["flat"])
+    errs = tail_nan(runs[0]["flat"], n, "acc") + tail_nan(lin_flat, c, "lin") + determinism(runs, ["flat"])
     if self_pair:
-        e, res = _exact(acc, acc0, "acc after comparing each image with itself")
+        e, res = exact(acc, acc0, "acc after comparing each image with itself")
         return errs + e, res
     A = fa[:, :c].double().reshape(n, hw, c)
     B = fb[:, :c].double().reshape(n, hw, c)
@@ -417,7 +389,7 @@ def replay_lpips_layer(R, f, self_pair=False, calls=1):
     for _ in range(calls):
         r = r + D
         bound = bound + E + EPS24 * r.abs()
-    e, res = _worst(ratio(acc, r, bound), ("image",), f" (hw {hw}, c {c}, {calls} call(s))")
+    e, res = worst_at(ratio(acc, r, bound), ("image",), f" (hw {hw}, c {c}, {calls} call(s))")
     return errs + e, res
 
 
@@ -441,13 +413,13 @@ def replay_ssim(R, f, inputs="noise"):
     x, y = _ssim_images(R, n, c, h, w, inputs)
 
     def fresh():
-        wf, ws = _buf(R, n * tiles, torch.float32)
-        of, o = _buf(R, n, torch.float32)
+        wf, ws = flat_buf(R, n * tiles, torch.float32)
+        of, o = flat_buf(R, n, torch.float32)
         return dict(wf=wf, ws=ws, of=of, out=o)
-    runs = _twice(lambda b: lib.call("ladi_ssim_f32", _P(x), _P(y), n, c, h, w, _P(b["ws"]), _P(b["out"]), R.stream), fresh)
-    errs = _tail_nan(runs[0]["wf"], n * tiles, "ws") + _tail_nan(runs[0]["of"], n, "out") + _determinism(runs, ["wf", "of"])
+    runs = twice(lambda b: lib.call("ladi_ssim_f32", ptr(x), ptr(y), n, c, h, w, ptr(b["ws"]), ptr(b["out"]), R.stream), fresh)
+    errs = tail_nan(runs[0]["wf"], n * tiles, "ws") + tail_nan(runs[0]["of"], n, "out") + determinism(runs, ["wf", "of"])
     r, bound = ssim_expect(x.double(), y.double())
-    e, res = _worst(ratio(runs[0]["out"], r, bound), ("image",), f" ({h}x{w}, c {c}, {tiles} partials, {inputs})")
+    e, res = worst_at(ratio(runs[0]["out"], r, bound), ("image",), f" ({h}x{w}, c {c}, {tiles} partials, {inputs})")
     return errs + e, res
 
 
@@ -467,18 +439,18 @@ def replay_resize_tf1(R, f, inputs="noise"):
     cnt = n * c * oh * ow
 
     def fresh():
-        flat, o = _buf(R, cnt, torch.float32)
+        flat, o = flat_buf(R, cnt, torch.float32)
         return dict(flat=flat, out=o)
-    runs = _twice(lambda b: lib.call("ladi_resize_tf1_u8", _P(x), n, c, h, w, oh, ow, _P(b["out"]), R.stream), fresh)
-    errs = _tail_nan(runs[0]["flat"], cnt, "output") + _determinism(runs, ["flat"])
+    runs = twice(lambda b: lib.call("ladi_resize_tf1_u8", ptr(x), n, c, h, w, oh, ow, ptr(b["out"]), R.stream), fresh)
+    errs = tail_nan(runs[0]["flat"], cnt, "output") + determinism(runs, ["flat"])
     y = runs[0]["out"].view(n, c, oh, ow)
     if (oh, ow) == (h, w):  # identity: sample positions are integers, the output is the texels themselves
-        e, res = _exact(y, resize_texels(x).float(), "identity resize against torch's fp32 (x * 255).byte()")
+        e, res = exact(y, resize_texels(x).float(), "identity resize against torch's fp32 (x * 255).byte()")
         return errs + e, res
     worst = (0.0, "")
-    for b in _pick_images(n, cnt * 16):
+    for b in pick(n, cnt * 16, 1 << 28):
         r, bound = resize_expect(x[b:b + 1], oh, ow)
-        e, res = _worst(ratio(y[b:b + 1], r, bound)[0], ("channel", "y", "x"), f" of image {b}")
+        e, res = worst_at(ratio(y[b:b + 1], r, bound)[0], ("channel", "y", "x"), f" of image {b}")
         errs += e
         worst = max(worst, res)
     return errs, worst
@@ -557,23 +529,21 @@ def test_metrics_census_integrity():
 def test_metrics_census_rejects_unknown_entry_point():
     """A workload that records an entry point without a SCHEMA row next to a known one: the census reports it, the integrity check fails."""
     known = ("ladi_resize_tf1_u8", (C.c_void_p(16), 1, 3, 8, 8, 4, 4, C.c_void_p(32), C.c_void_p(0)))
-    desc, calls, unknown, _ = collect([("fake workload", lambda: [known, ("ladi_not_in_the_schema", (C.c_void_p(16), 3, C.c_void_p(0)))])])
+    desc, calls, unknown, _ = metrics_collect([("fake workload", lambda: [known, ("ladi_not_in_the_schema", (C.c_void_p(16), 3, C.c_void_p(0)))])])
     assert unknown == ["ladi_not_in_the_schema"] and [d["kind"] for d in desc.values()] == ["resize_tf1"]
     with pytest.raises(AssertionError, match="ladi_not_in_the_schema"):
         assert_all_known(unknown)
 
 
 # ================================================================================================================ CPU: the bounds have teeth
-def _check(y, r, bound):
-    return float(ratio(y, r, bound).max())
 
 
 def test_teeth_exclude_pad_counts_padding():
     g = torch.Generator().manual_seed(11)
     x = (torch.randn((2, 16, 9, 7), generator=g) * 2).bfloat16().float()
     r, bound = pool_expect(x.double(), 3, 1, 1, POOL_EXCL)
-    assert _check(F.avg_pool2d(x, 3, 1, 1, count_include_pad=False).bfloat16(), r, bound) <= 1
-    assert _check(F.avg_pool2d(x, 3, 1, 1, count_include_pad=True).bfloat16(), r, bound) > 1  # 1. padding counted at the border
+    assert max_ratio(F.avg_pool2d(x, 3, 1, 1, count_include_pad=False).bfloat16(), r, bound) <= 1
+    assert max_ratio(F.avg_pool2d(x, 3, 1, 1, count_include_pad=True).bfloat16(), r, bound) > 1  # 1. padding counted at the border
 
 
 @pytest.mark.parametrize("kh,sh,ph", [(11, 4, 2), (3, 2, 1)])
@@ -589,8 +559,8 @@ def test_teeth_pixel_affine_on_padding(kh, sh, ph):
     honest = im2col_ref(((x - shift.view(-1, 1, 1)) / scale.view(-1, 1, 1)).bfloat16().permute(0, 2, 3, 1), *geo)
     xp = F.pad(x, (ph, ph, ph, ph))  # 2. zero padding first, then the affine: the padding becomes -shift / scale
     faulty = im2col_ref(((xp - shift.view(-1, 1, 1)) / scale.view(-1, 1, 1)).bfloat16().permute(0, 2, 3, 1), kh, kh, sh, sh, 0, 0, geo[6])
-    assert _check(honest, r, bound) <= 1
-    assert _check(faulty, r, bound) > 1
+    assert max_ratio(honest, r, bound) <= 1
+    assert max_ratio(faulty, r, bound) > 1
 
 
 def _ssim_emulate(x, y, extent=0, drop_last_tile=False):
@@ -619,9 +589,9 @@ def test_teeth_ssim():
     x = torch.rand((2, 3, 64, 48), generator=g)
     y = (x + 0.15 * torch.randn(x.shape, generator=g)).clamp(0.0, 1.0)
     r, bound = ssim_expect(x.double(), y.double())
-    assert _check(_ssim_emulate(x, y), r, bound) <= 1
-    assert _check(_ssim_emulate(x, y, extent=1), r, bound) > 1  # 3. valid extent one too large
-    assert _check(_ssim_emulate(x, y, drop_last_tile=True), r, bound) > 1  # 4. the last partial tile dropped
+    assert max_ratio(_ssim_emulate(x, y), r, bound) <= 1
+    assert max_ratio(_ssim_emulate(x, y, extent=1), r, bound) > 1  # 3. valid extent one too large
+    assert max_ratio(_ssim_emulate(x, y, drop_last_tile=True), r, bound) > 1  # 4. the last partial tile dropped
 
 
 def test_teeth_lpips_remainder_pixels():
@@ -637,8 +607,8 @@ def test_teeth_lpips_remainder_pixels():
         rb = 1.0 / ((b * b).sum(-1, keepdim=True).sqrt() + 1e-10)
         d = (lin * (a * ra - b * rb) ** 2).sum(-1)
         return (d[:, :hw - hw % 16] if drop else d).sum(1) / hw
-    assert _check(emulate(False), D, E) <= 1
-    assert _check(emulate(True), D, E) > 1  # 5. the hw % 16 remainder pixels dropped
+    assert max_ratio(emulate(False), D, E) <= 1
+    assert max_ratio(emulate(True), D, E) > 1  # 5. the hw % 16 remainder pixels dropped
 
 
 @pytest.mark.parametrize("fault", ["round", "half_pixel"])
@@ -665,12 +635,11 @@ def test_teeth_resize_tf1(fault):
         top = at(y0, x0) + (at(y0, x1) - at(y0, x0)) * lx
         bot = at(y1, x0) + (at(y1, x1) - at(y1, x0)) * lx
         return top + (bot - top) * ly.view(-1, 1)
-    assert _check(emulate(), r, bound) <= 1
-    assert _check(emulate(fault), r, bound) > 1  # 6. rounding instead of truncating / 7. half-pixel centres
+    assert max_ratio(emulate(), r, bound) <= 1
+    assert max_ratio(emulate(fault), r, bound) > 1  # 6. rounding instead of truncating / 7. half-pixel centres
 
 
 # ================================================================================================================ CPU: placement rules
-A = 1 << 20  # a fake, 256-byte aligned device address; never dereferenced
 # (id, entry point, arguments with pointers as ints, expected message or None = the checks pass and the launch fails for lack of a device)
 _IM2COL_NHWC = lambda x=A, out=A: ("ladi_im2col_bf16", [x, 0, 1, 8, 4, 4, 8, 3, 3, 1, 1, 1, 1, 0, 0, out, 72])  # noqa: E731
 _IM2COL_PX = lambda x=A, sh=A, sc=A + 64, out=A: ("ladi_im2col_bf16", [x, 1, 1, 3, 8, 8, 0, 3, 3, 2, 2, 0, 0, sh, sc, out, 64])  # noqa: E731
@@ -708,37 +677,11 @@ PLACEMENT = [
     ("resize out", *_RESIZE(out=A + 2), "out 0x100002 must be 4-byte aligned"),
     ("resize ok", *_RESIZE(x=A + 4, out=A + 4), None),
 ]
-_CHILD = r"""
-import ctypes as C, json, sys
-sys.path.insert(0, sys.argv[1])
-from ladi_vton_b200 import lib
-L = lib.load()
-res = []
-for name, args in json.loads(sys.argv[2]):
-    fn = getattr(L, name)
-    rc = fn(*[C.c_void_p(a) if t is C.c_void_p else a for a, t in zip(args, fn.argtypes)], None)
-    res.append([rc, L.ladi_last_error().decode()])
-print(json.dumps(res))
-"""
 
 
 def test_placement_rules_without_a_device():
-    """Each rule rejects with LADI_ERR_INVALID and a message naming the operand; a placement that meets the rules passes the checks and
-    then fails with LADI_ERR_CUDA, because the child process sees no device: no call here can launch a kernel."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, CUDA_VISIBLE_DEVICES="")
-    out = subprocess.run([sys.executable, "-c", _CHILD, root, json.dumps([[n, a] for _, n, a, _ in PLACEMENT])], env=env, capture_output=True,
-                         text=True, timeout=120)
-    assert out.returncode == 0, out.stderr
-    res = json.loads(out.stdout.strip().splitlines()[-1])
-    bad = []
-    for (what, name, _, want), (rc, msg) in zip(PLACEMENT, res):
-        if want is None:
-            if rc != 2:
-                bad.append(f"{what}: rc {rc} ({msg}); expected the checks to pass and the launch to fail without a device")
-        elif rc != 1 or want not in msg:
-            bad.append(f"{what}: rc {rc} ({msg}); expected LADI_ERR_INVALID with '{want}'")
-    assert not bad, "\n".join(bad)
+    """The placement rules of the metrics entry points (PLACEMENT), checked in a process that sees no device."""
+    check_placement(PLACEMENT)
 
 
 # ================================================================================================================ GPU: replay

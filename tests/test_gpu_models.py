@@ -11,12 +11,9 @@ import numpy as np
 import pytest
 import torch
 
+from kernel_check import rel_l2
+
 pytestmark = pytest.mark.gpu
-
-
-def rel_l2(y, ref):
-    y, ref = y.detach().float().cpu(), ref.detach().float().cpu()
-    return ((y - ref).norm() / ref.norm().clamp_min(1e-12)).item()
 
 
 @pytest.fixture(scope="module")

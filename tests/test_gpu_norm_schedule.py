@@ -3,7 +3,7 @@
 `ladi_groupnorm_plan` and `ladi_layernorm_plan` report the grids the launches would run; they share the validation-and-policy function
 with the launches and need no device.  Every GPU case first asserts, through the query at the device's SM count, the plan it means to
 exercise (the expectations are those of a 132-SM H100 SXM; on another SM count only the float64 checks run).  It then runs the call the
-way tests/test_gpu_workload_census.py replays the workload's: every input pitch gap is NaN, the output is NaN over its full pitch plus
+way the workload census replays the workload's (tests/kernel_check.py): every input pitch gap is NaN, the output is NaN over its full pitch plus
 TAIL rows, afterwards every owned element is finite and every other one still NaN, a second run is bit-identical, and every element is
 within a float64 bound.
 
@@ -14,7 +14,7 @@ bound allows near the many outputs close to zero.  One characterisation case at 
 the one-pass fp32 variance against the census bound, which prices it in.
 
 LayerNorm computes its statistics in two passes (mean, then the sum of squared deviations), so it gets its own bound, `ln_expect`:
-  d_mean = delta (|mean| + sd), delta = C_ACC sqrt(C) 2^-24    the fp32 sum of C bf16 values, divided by C (as in the census);
+  d_mean = delta (|mean| + sd), delta = C_ACC sqrt(C) 2^-24    the fp32 sum of C bf16 values, divided by C (as in norm_expect);
   var:  the sum of C non-negative squares of fp32 deviations: relative error delta from the accumulation, 2^-23 from forming and
         squaring each deviation, plus (d_mean / sd)^2 because the deviations are taken from the computed mean -- no mean^2 / var term;
   d_rstd = 1.5 (delta + 2^-23 + d_mean^2 / (var + eps)) + 2^-22  (half the relative variance error through rsqrt, tripled for margin,
@@ -34,20 +34,10 @@ import zlib
 import pytest
 import torch
 
-from test_gpu_workload_census import C_ACC, EPS24, U_BF16, Replay, _bitwise_equal, _layout, norm_expect, ratio
+from kernel_check import (C_ACC, EPS24, TAIL, U_BF16, Replay, addr, argworst, determinism, ladi_lib, launches, layout, norm_expect, override,
+                          plan_query, ratio, sms, twice)
 
-TAIL = 3  # NaN rows after the output that no call may write
-BASE = 1 << 40  # fake device addresses for the queries: they dereference nothing
 EPS = 1e-6
-
-
-def _lib():
-    from ladi_vton_b200 import lib
-    return lib
-
-
-def _addr(slot, byte_off=0):
-    return BASE + slot * (1 << 32) + byte_off
 
 
 GN_FIELDS = ("chunks", "gsplit", "block_channels", "lanes_v", "k", "px_per_chunk", "px_per_block", "apply_blocks", "dv", "dp", "slices")
@@ -56,18 +46,9 @@ GN_FIELDS = ("chunks", "gsplit", "block_channels", "lanes_v", "k", "px_per_chunk
 def gn_args(c0, c1, n, hw, groups, **kw):
     """The arguments of ladi_groupnorm_apply (without the stream) on fake 256-byte aligned addresses; kw overrides by name, *_off adds
     a byte offset to a pointer."""
-    return _override(dict(x0=_addr(1), c0=c0, pitch0=c0, x1=_addr(2) if c1 else None, c1=c1, pitch1=c1, n=n, hw=hw, groups=groups,
-                          ws=_addr(3), gamma=_addr(4), beta=_addr(5), eps=EPS, silu=1, add=None, add_pitch=0, out=_addr(6),
+    return override(dict(x0=addr(1), c0=c0, pitch0=c0, x1=addr(2) if c1 else None, c1=c1, pitch1=c1, n=n, hw=hw, groups=groups,
+                          ws=addr(3), gamma=addr(4), beta=addr(5), eps=EPS, silu=1, add=None, add_pitch=0, out=addr(6),
                           out_pitch=c0 + c1), kw)
-
-
-def _override(a, kw):
-    for k, v in kw.items():
-        if k.endswith("_off"):
-            a[k[:-4]] += v
-        else:
-            a[k] = v
-    return a
 
 
 _GN_ORDER = ("x0", "c0", "pitch0", "x1", "c1", "pitch1", "n", "hw", "groups", "ws", "gamma", "beta", "eps", "silu", "add", "add_pitch", "out",
@@ -76,14 +57,7 @@ _GN_ORDER = ("x0", "c0", "pitch0", "x1", "c1", "pitch1", "n", "hw", "groups", "w
 
 def gn_query(a, sms):
     """-> (plan dict, "") or (None, error message)."""
-    lib = _lib()
-    L = lib.load()
-    pl = lib.GroupNormPlan()
-    rc = L.ladi_groupnorm_plan(*[a[k] for k in _GN_ORDER], sms, C.byref(pl))
-    if rc:
-        assert rc == 1, rc
-        return None, L.ladi_last_error().decode()
-    return {f: getattr(pl, f) for f in GN_FIELDS}, ""
+    return plan_query("ladi_groupnorm_plan", ladi_lib().GroupNormPlan, [a[k] for k in _GN_ORDER] + [sms], GN_FIELDS)
 
 
 def gn_plan(c0, c1, n, hw, groups, sms, **kw):
@@ -92,20 +66,15 @@ def gn_plan(c0, c1, n, hw, groups, sms, **kw):
     return p
 
 
+_LN_ORDER = ("x", "x_pitch", "rows", "c", "gamma", "beta", "eps", "out", "out_pitch")
+
+
 def ln_args(rows, c, **kw):
-    return _override(dict(x=_addr(1), x_pitch=c, rows=rows, c=c, gamma=_addr(2), beta=_addr(3), eps=1e-5, out=_addr(4), out_pitch=c), kw)
+    return override(dict(x=addr(1), x_pitch=c, rows=rows, c=c, gamma=addr(2), beta=addr(3), eps=1e-5, out=addr(4), out_pitch=c), kw)
 
 
 def ln_query(a):
-    lib = _lib()
-    L = lib.load()
-    pl = lib.LayerNormPlan()
-    rc = L.ladi_layernorm_plan(a["x"], a["x_pitch"], a["rows"], a["c"], a["gamma"], a["beta"], a["eps"], a["out"], a["out_pitch"], 0,
-                               C.byref(pl))
-    if rc:
-        assert rc == 1, rc
-        return None, L.ladi_last_error().decode()
-    return dict(T=pl.T, vpl=pl.vpl, rows_per_block=pl.rows_per_block, blocks=pl.blocks), ""
+    return plan_query("ladi_layernorm_plan", ladi_lib().LayerNormPlan, [a[k] for k in _LN_ORDER] + [0], ("T", "vpl", "rows_per_block", "blocks"))
 
 
 # ================================================================================================================ CPU: plan tables
@@ -181,9 +150,9 @@ GN_REJECT = [  # (name, overrides, word the message must contain)
     ("hw zero", dict(hw=0), "hw > 0"),
     ("ws null", dict(ws=None), "ws"),
     ("out misaligned", dict(out_off=8), "out"),
-    ("add misaligned", dict(add=_addr(7, 8), add_pitch=384), "add"),
-    ("add_pitch odd", dict(add=_addr(7), add_pitch=385), "add_pitch"),
-    ("add_pitch below C", dict(add=_addr(7), add_pitch=376), "add_pitch"),
+    ("add misaligned", dict(add=addr(7, 8), add_pitch=384), "add"),
+    ("add_pitch odd", dict(add=addr(7), add_pitch=385), "add_pitch"),
+    ("add_pitch below C", dict(add=addr(7), add_pitch=376), "add_pitch"),
     ("gamma null", dict(gamma=None), "gamma"),
     ("beta null", dict(beta=None), "beta"),
     ("out_pitch below C", dict(out_pitch=376), "out_pitch"),
@@ -192,15 +161,15 @@ GN_REJECT = [  # (name, overrides, word the message must contain)
 
 @pytest.mark.parametrize("name,kw,word", GN_REJECT, ids=[r[0] for r in GN_REJECT])
 def test_gn_placement_rejected(name, kw, word):
-    p, err = gn_query(_override(gn_args(320, 64, 2, 100, 32), kw), 132)
+    p, err = gn_query(override(gn_args(320, 64, 2, 100, 32), kw), 132)
     assert p is None, f"{name}: accepted"
     assert word in err, err
 
 
 GN_ACCEPT = [
-    ("x1 unaligned but unused", dict(c1=0, x1=_addr(2, 2), pitch1=0)),
+    ("x1 unaligned but unused", dict(c1=0, x1=addr(2, 2), pitch1=0)),
     ("gamma / beta 4-byte aligned (scalar loads)", dict(gamma_off=4, beta_off=12)),
-    ("add aligned, wider pitch", dict(add=_addr(7, 16), add_pitch=400)),
+    ("add aligned, wider pitch", dict(add=addr(7, 16), add_pitch=400)),
     ("pitches above the widths", dict(pitch0=328, pitch1=72, out_pitch=400)),
     ("add_pitch ignored without add", dict(add_pitch=3)),
 ]
@@ -208,7 +177,7 @@ GN_ACCEPT = [
 
 @pytest.mark.parametrize("name,kw", GN_ACCEPT, ids=[r[0] for r in GN_ACCEPT])
 def test_gn_placement_accepted(name, kw):
-    p, err = gn_query(_override(gn_args(320, 64, 2, 100, 32), kw), 132)
+    p, err = gn_query(override(gn_args(320, 64, 2, 100, 32), kw), 132)
     assert p is not None, err
 
 
@@ -228,7 +197,7 @@ LN_REJECT = [
 
 @pytest.mark.parametrize("name,kw,word", LN_REJECT, ids=[r[0] for r in LN_REJECT])
 def test_ln_placement_rejected(name, kw, word):
-    p, err = ln_query(_override(ln_args(100, 320), kw))
+    p, err = ln_query(override(ln_args(100, 320), kw))
     assert p is None, f"{name}: accepted"
     assert word in err, err
 
@@ -247,7 +216,7 @@ def _gn_data(g, hw, C, groups, offset=3.0, sentinels=True):
     mu = s * (torch.rand(groups, generator=g, dtype=torch.float64) * 2 - 1) * offset
     z = torch.randn((hw, C), generator=g, dtype=torch.float64)
     if sentinels:
-        chunks = _lib().load().ladi_groupnorm_chunks(hw)
+        chunks = ladi_lib().load().ladi_groupnorm_chunks(hw)
         per = -(-hw // chunks)
         for c in range(chunks):
             p0, p1 = c * per, min(hw, (c + 1) * per)
@@ -264,7 +233,7 @@ def _emulate_gn(x, groups, gamma, beta, eps, silu, add=None, fault=None):
     and over chunks, one-pass variance, y = x a + b (a = rstd gamma, b = beta - mean a), SiLU as h (1 + tanh h), then + add."""
     hw, Cc = x.shape
     cpg = Cc // groups
-    chunks = _lib().load().ladi_groupnorm_chunks(hw)
+    chunks = ladi_lib().load().ladi_groupnorm_chunks(hw)
     per = -(-hw // chunks)
     xf = x.float()
     grp = torch.arange(Cc) // cpg
@@ -412,8 +381,6 @@ def test_ln_checker_teeth(c):
 
 
 # ================================================================================================================ GPU: GroupNorm
-def _sms(dev):
-    return torch.cuda.get_device_properties(dev).multi_processor_count
 
 
 def _gn_inputs(R, n, hw, c0, c1, groups, offset):
@@ -425,7 +392,7 @@ def _gn_inputs(R, n, hw, c0, c1, groups, offset):
 
 def run_gn(R, c0, c1, n, hw, groups, silu=1, add=False, offset=3.0, expect=None):
     """One GroupNorm call (stats + apply) checked as the module docstring says; -> worst err/bound."""
-    lib = _lib()
+    lib = ladi_lib()
     L = lib.load()
     Ct = c0 + c1
     p0, p1, op, ap = c0 + 8, c1 + 24 if c1 else 0, Ct + 16, Ct + 40  # distinct pitches, all with NaN gaps
@@ -436,36 +403,35 @@ def run_gn(R, c0, c1, n, hw, groups, silu=1, add=False, offset=3.0, expect=None)
     addt = R.poisoned(n * hw, ap, R.randn(n * hw, Ct)) if add else None
     P = lambda t: t.data_ptr() if t is not None else None
     chunks = L.ladi_groupnorm_chunks(hw)
-    outs = []
-    for _ in range(2):
-        ws = torch.full((n * chunks * groups * 2,), float("nan"), dtype=torch.float32, device=R.dev)
-        o = R.poisoned(n * hw + TAIL, op)
-        a = dict(x0=P(x0), c0=c0, pitch0=p0, x1=P(x1), c1=c1, pitch1=p1, n=n, hw=hw, groups=groups, ws=P(ws), gamma=P(gamma), beta=P(beta),
-                 eps=EPS, silu=silu, add=P(addt), add_pitch=ap if add else 0, out=P(o), out_pitch=op)
+    plan = None
+
+    def call(b):
+        nonlocal plan
+        a = dict(x0=P(x0), c0=c0, pitch0=p0, x1=P(x1), c1=c1, pitch1=p1, n=n, hw=hw, groups=groups, ws=P(b["ws"]), gamma=P(gamma), beta=P(beta),
+                 eps=EPS, silu=silu, add=P(addt), add_pitch=ap if add else 0, out=P(b["out"]), out_pitch=op)
         plan, err = gn_query(a, 0)  # what runs on this device
         assert plan is not None, err
         if expect:  # the branch the shape reaches on a 132-SM H100 SXM, asserted on any device; there, it is also what runs
             p132, _ = gn_query(a, 132)
             assert {k: p132[k] for k in expect} == expect, f"plan at 132 SMs {p132}, expected {expect}"
-            if _sms(R.dev) == 132:
+            if sms(R.dev) == 132:
                 assert plan == p132
-        lib.call("ladi_groupnorm_stats", P(x0), c0, p0, P(x1), c1, p1, n, hw, groups, P(ws), R.stream)
+        lib.call("ladi_groupnorm_stats", P(x0), c0, p0, P(x1), c1, p1, n, hw, groups, P(b["ws"]), R.stream)
         lib.call("ladi_groupnorm_apply", *[a[k] for k in _GN_ORDER], R.stream)
-        outs.append(o)
-    torch.cuda.synchronize()
-    errs = _layout(outs[0][:n * hw], Ct, "output")
+    runs = twice(call, lambda: dict(ws=torch.full((n * chunks * groups * 2,), float("nan"), dtype=torch.float32, device=R.dev),
+                                    out=R.poisoned(n * hw + TAIL, op)))
+    out = runs[0]["out"]
+    errs = layout(out, 0, Ct, "output", rows=n * hw)
     assert not errs, errs
-    assert bool(torch.isnan(outs[0][n * hw:].float()).all()), "wrote past the last image"
-    assert _bitwise_equal(outs[0], outs[1]), "two runs differ bitwise"
+    errs = determinism(runs, ["out"])
+    assert not errs, errs
     worst = 0.0
     for b in range(n) if n * hw * Ct <= 1 << 26 else (0, n - 1):
         xb = torch.cat([v0[b * hw:(b + 1) * hw], v1[b * hw:(b + 1) * hw]], dim=1) if c1 else v0[b * hw:(b + 1) * hw]
         ab = addt[b * hw:(b + 1) * hw, :Ct] if add else None
         r, bound = _gn_ref(xb, groups, gamma, beta, EPS, silu, ab)
-        q = ratio(outs[0][b * hw:(b + 1) * hw, :Ct], r, bound)
-        qm = float(q.max())
+        qm, (p, c) = argworst(ratio(out[b * hw:(b + 1) * hw, :Ct], r, bound))
         if qm > 1.0:
-            p, c = (int(t) for t in torch.unravel_index(q.argmax(), q.shape))
             pytest.fail(f"image {b}: err/bound {qm:.3g} at pixel {p}, channel {c} (group {c // (Ct // groups)}); plan {plan}")
         worst = max(worst, qm)
     return worst
@@ -534,32 +500,30 @@ def test_groupnorm_one_pass_characterisation(cuda):
 
 # ================================================================================================================ GPU: LayerNorm
 def run_ln(R, rows, c, expect=None, max_offset=30.0):
-    lib = _lib()
+    lib = ladi_lib()
     xp, op = c + 24, c + 8
     g = torch.Generator(device=R.dev).manual_seed(rows * 4099 + c)
     xv = _ln_data(g, rows, c, max_offset=max_offset, dev=R.dev)
     gamma, beta = _ln_affine(g, c, dev=R.dev)
     x = R.poisoned(rows, xp, xv)
-    outs = []
-    for _ in range(2):
-        o = R.poisoned(rows + TAIL, op)
-        a = ln_args(rows, c, x=x.data_ptr(), x_pitch=xp, gamma=gamma.data_ptr(), beta=beta.data_ptr(), out=o.data_ptr(), out_pitch=op)
+    plan = None
+
+    def call(b):
+        nonlocal plan
+        a = ln_args(rows, c, x=x.data_ptr(), x_pitch=xp, gamma=gamma.data_ptr(), beta=beta.data_ptr(), out=b["out"].data_ptr(), out_pitch=op)
         plan, err = ln_query(a)
         assert plan is not None, err
         if expect:
             assert {k: plan[k] for k in expect} == expect, f"plan {plan}, expected {expect}"
         lib.call("ladi_layernorm", a["x"], xp, rows, c, a["gamma"], a["beta"], a["eps"], a["out"], op, R.stream)
-        outs.append(o)
-    torch.cuda.synchronize()
-    errs = _layout(outs[0][:rows], c, "output")
+    runs = twice(call, lambda: dict(out=R.poisoned(rows + TAIL, op)))
+    errs = layout(runs[0]["out"], 0, c, "output", rows=rows)
     assert not errs, errs
-    assert bool(torch.isnan(outs[0][rows:].float()).all()), "wrote past the last row"
-    assert _bitwise_equal(outs[0], outs[1]), "two runs differ bitwise"
+    errs = determinism(runs, ["out"])
+    assert not errs, errs
     r, bound = ln_expect(xv.double(), gamma.double(), beta.double(), 1e-5)
-    q = ratio(outs[0][:rows, :c], r, bound)
-    worst = float(q.max())
+    worst, (i, j) = argworst(ratio(runs[0]["out"][:rows, :c], r, bound))
     if worst > 1.0:
-        i, j = (int(t) for t in torch.unravel_index(q.argmax(), q.shape))
         pytest.fail(f"err/bound {worst:.3g} at row {i}, column {j}; plan {plan}")
     return worst
 
@@ -586,14 +550,12 @@ LN_ROWS = {"1": lambda rpw, rpb, s: 1, "rpw-1": lambda rpw, rpb, s: max(1, rpw -
 def test_layernorm_row_counts(cuda, c, rows):
     T, _ = _ln_shape(c)
     rpw, rpb = 32 // T, 8 * 32 // T
-    n = LN_ROWS[rows](rpw, rpb, _sms(cuda))
+    n = LN_ROWS[rows](rpw, rpb, sms(cuda))
     worst = run_ln(Replay(cuda, n), n, c, expect=dict(T=T, blocks=-(-n // rpb)))
     print(f"\nLayerNorm C {c}, {n} rows: worst err/bound {worst:.3g}")
 
 
 # ================================================================================================================ GPU: placement
-def _launches():
-    return _lib().load().ladi_launch_count()
 
 
 GN_GPU_REJECT = [("x0 misaligned", "x0", 8), ("x1 misaligned", "x1", 8), ("out misaligned", "out", 8), ("add misaligned", "add", 8),
@@ -605,7 +567,7 @@ GN_GPU_REJECT = [("x0 misaligned", "x0", 8), ("x1 misaligned", "x1", 8), ("out m
 def test_groupnorm_placement_rejected_on_device(cuda, name, what, off):
     """The query rejects the placement first; only then do the launching calls see it, and they return the same error, launch nothing
     and leave the output NaN."""
-    L = _lib().load()
+    L = ladi_lib().load()
     n, hw, c0, c1, G = 2, 100, 256, 64, 32
     R = Replay(cuda, 5)
     x0 = R.poisoned(n * hw + 1, c0 + 8, R.randn(n * hw + 1, c0))
@@ -623,14 +585,14 @@ def test_groupnorm_placement_rejected_on_device(cuda, name, what, off):
         a[what] += off
     plan, err = gn_query(a, 0)
     assert plan is None and what in err, (plan, err)
-    before = _launches()
+    before = launches()
     if what in ("x0", "x1", "pitch0"):
         assert L.ladi_groupnorm_stats(a["x0"], c0, a["pitch0"], a["x1"], c1, a["pitch1"], n, hw, G, a["ws"], None) == 1
         assert L.ladi_last_error().decode() == err
     assert L.ladi_groupnorm_apply(*[a[k] for k in _GN_ORDER], None) == 1
     assert L.ladi_last_error().decode() == err
     torch.cuda.synchronize()
-    assert _launches() == before
+    assert launches() == before
     assert bool(torch.isnan(o.float()).all())
 
 
@@ -640,7 +602,7 @@ LN_GPU_REJECT = [("x misaligned", "x"), ("out misaligned", "out"), ("gamma misal
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,what", LN_GPU_REJECT, ids=[r[0] for r in LN_GPU_REJECT])
 def test_layernorm_placement_rejected_on_device(cuda, name, what):
-    L = _lib().load()
+    L = ladi_lib().load()
     rows, c = 100, 320
     R = Replay(cuda, 6)
     x = R.poisoned(rows + 1, c, R.randn(rows + 1, c))
@@ -650,9 +612,9 @@ def test_layernorm_placement_rejected_on_device(cuda, name, what):
     a[what] += 4 if what in ("gamma", "beta") else 8
     plan, err = ln_query(a)
     assert plan is None and what in err, (plan, err)
-    before = _launches()
+    before = launches()
     assert L.ladi_layernorm(a["x"], c, rows, c, a["gamma"], a["beta"], a["eps"], a["out"], c, None) == 1
     assert L.ladi_last_error().decode() == err
     torch.cuda.synchronize()
-    assert _launches() == before
+    assert launches() == before
     assert bool(torch.isnan(o.float()).all())

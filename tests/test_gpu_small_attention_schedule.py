@@ -6,7 +6,7 @@ loads only the keys its last row sees.  `cls_attention_kernel` (`ladi_cls_attent
 over tokens for the scores and over head columns for P.V.  `ladi_attention_small_plan` / `ladi_cls_attention_plan` report what the
 launches run; they share the validation-and-policy function with the launches and need no device.  Every GPU case first asserts,
 through the query at 132 SMs, the plan it means to exercise (on a 132-SM H100 SXM that is also the plan that runs).  It then goes
-through the census checkers (`check_attention_small`, `check_cls`): every input pitch gap and the gaps between images are NaN, the
+through the census checkers (`check_attention_small`, `check_cls` in tests/kernel_check.py): every input pitch gap and the gaps between images are NaN, the
 output is NaN over its full pitch, between images and in a tail, afterwards exactly the rows and columns the call owns are finite, a
 second run is bit-identical, and every query row of every image is within the float64 bound (attn_expect with P in fp32).
 
@@ -15,7 +15,6 @@ row's maximum sits on its diagonal and the last keys dominate), "large" (scores 
 
 The CPU tests pin the plan tables and every placement rule through the queries, and show the checkers have teeth: a float32 emulation
 of each kernel's block and warp split, driven by the queried plan, passes, and four simulated faults are rejected."""
-import ctypes as C
 import time
 import zlib
 
@@ -23,31 +22,10 @@ import numpy as np
 import pytest
 import torch
 
-from test_gpu_glue_frontend_census import check_attention_small, small_attn_expect
-from test_gpu_workload_census import Replay, _attn_ref, attn_expect, check_cls, ratio
+from kernel_check import (NAN, SMS, Replay, addr, attn_expect, attn_ref, check_attention_small, check_cls, ladi_lib, launches, override,
+                          plan_query, ratio, small_attn_expect, sms)
 
-SMS = 132  # H100 SXM
-BASE = 1 << 40  # fake device addresses for the queries: they dereference nothing
-NAN = float("nan")
 OPTIN = 48 * 1024
-
-
-def _lib():
-    from ladi_vton_b200 import lib
-    return lib
-
-
-def _addr(slot, byte_off=0):
-    return BASE + slot * (1 << 32) + byte_off
-
-
-def _override(a, kw):
-    for k, v in kw.items():
-        if k.endswith("_off"):
-            a[k[:-4]] += v
-        else:
-            a[k] = v
-    return a
 
 
 # ================================================================================================================ queries
@@ -59,24 +37,13 @@ def sa_desc(B, heads, nq, nkv, hd, causal=0, **kw):
     """ladi_attention_small's arguments in the glue census's field names: dense [B, n, heads*hd] operands on fake 256-byte aligned
     addresses; kw overrides by name, *_off adds a byte offset to a pointer."""
     Cw = heads * hd
-    return _override(dict(q=_addr(1), k=_addr(2), v=_addr(3), out=_addr(4), B=B, heads=heads, nq=nq, nkv=nkv, hd=hd, qp=Cw, kp=Cw, vp=Cw,
+    return override(dict(q=addr(1), k=addr(2), v=addr(3), out=addr(4), B=B, heads=heads, nq=nq, nkv=nkv, hd=hd, qp=Cw, kp=Cw, vp=Cw,
                           op=Cw, qbs=nq * Cw, kbs=nkv * Cw, vbs=nkv * Cw, obs=nq * Cw, scale=hd ** -0.5, causal=causal), kw)
-
-
-def _query(fn, args, sms):
-    lib = _lib()
-    L = lib.load()
-    pl = lib.SmallAttnPlan()
-    rc = getattr(L, fn)(*args, sms, C.byref(pl))
-    if rc:
-        assert rc == 1, rc
-        return None, L.ladi_last_error().decode()
-    return {f: getattr(pl, f) for f in PLAN_FIELDS}, ""
 
 
 def sa_query(d, sms=SMS):
     """-> (plan dict, "") or (None, error message)."""
-    return _query("ladi_attention_small_plan", [d[k] for k in SA_ORDER], sms)
+    return plan_query("ladi_attention_small_plan", ladi_lib().SmallAttnPlan, [d[k] for k in SA_ORDER] + [sms], PLAN_FIELDS)
 
 
 CLS_ORDER = ("q", "qp", "kv", "kvp", "batch", "tokens", "heads", "hd", "scale", "out", "op")
@@ -85,12 +52,12 @@ CLS_ORDER = ("q", "qp", "kv", "kvp", "batch", "tokens", "heads", "hd", "scale", 
 def cls_desc(B, T, heads, hd, **kw):
     """ladi_cls_attention's arguments in the workload census's field names (dense, fake addresses), overridden like sa_desc."""
     Cw = heads * hd
-    return _override(dict(q=_addr(1), qp=Cw, kv=_addr(2), kvp=2 * Cw, batch=B, tokens=T, heads=heads, hd=hd, scale=hd ** -0.5, out=_addr(3),
+    return override(dict(q=addr(1), qp=Cw, kv=addr(2), kvp=2 * Cw, batch=B, tokens=T, heads=heads, hd=hd, scale=hd ** -0.5, out=addr(3),
                           op=Cw), kw)
 
 
 def cls_query(d, sms=SMS):
-    return _query("ladi_cls_attention_plan", [d[k] for k in CLS_ORDER], sms)
+    return plan_query("ladi_cls_attention_plan", ladi_lib().SmallAttnPlan, [d[k] for k in CLS_ORDER] + [sms], PLAN_FIELDS)
 
 
 def sa_smem(hd, nkv):
@@ -185,7 +152,7 @@ SA_REJECT = [  # (name, overrides, word the message must contain)
 
 @pytest.mark.parametrize("name,kw,word", SA_REJECT, ids=[r[0] for r in SA_REJECT])
 def test_attention_small_placement_rejected(name, kw, word):
-    p, err = sa_query(_override(sa_desc(2, 2, 10, 20, 64), kw))
+    p, err = sa_query(override(sa_desc(2, 2, 10, 20, 64), kw))
     assert p is None, f"{name}: accepted"
     assert word in err, err
 
@@ -193,7 +160,7 @@ def test_attention_small_placement_rejected(name, kw, word):
 SA_ACCEPT = [
     ("q and out 4-byte aligned", dict(q_off=4, out_off=12)),
     ("k and v 16-byte aligned", dict(k_off=16, v_off=48)),
-    ("fused QKV", dict(k=_addr(1, 256), v=_addr(1, 512), qp=384, kp=384, vp=384, qbs=10 * 384 + 8, kbs=10 * 384 + 8, vbs=10 * 384 + 8)),
+    ("fused QKV", dict(k=addr(1, 256), v=addr(1, 512), qp=384, kp=384, vp=384, qbs=10 * 384 + 8, kbs=10 * 384 + 8, vbs=10 * 384 + 8)),
     ("input images overlap (batch stride 0)", dict(kbs=0, vbs=0)),
     ("out images with gaps", dict(obs=10 * 136 + 8, op=136)),
     ("one image: out_batch_stride unused", dict(B=1, obs=0)),
@@ -202,7 +169,7 @@ SA_ACCEPT = [
 
 @pytest.mark.parametrize("name,kw", SA_ACCEPT, ids=[r[0] for r in SA_ACCEPT])
 def test_attention_small_placement_accepted(name, kw):
-    p, err = sa_query(_override(sa_desc(2, 2, 10, 10 if "fused" in name else 20, 64), kw))
+    p, err = sa_query(override(sa_desc(2, 2, 10, 10 if "fused" in name else 20, 64), kw))
     assert p is not None, err
 
 
@@ -219,7 +186,7 @@ CLS_REJECT = [
 
 @pytest.mark.parametrize("name,kw,word", CLS_REJECT, ids=[r[0] for r in CLS_REJECT])
 def test_cls_placement_rejected(name, kw, word):
-    p, err = cls_query(_override(cls_desc(2, 30, 2, 80), kw))
+    p, err = cls_query(override(cls_desc(2, 30, 2, 80), kw))
     assert p is None, f"{name}: accepted"
     assert word in err, err
 
@@ -236,7 +203,7 @@ def test_production_placements_accepted():
     output, a fresh dense output) and csrc/engine.cu's (the same on workspace blocks of 256 bytes), and the adapter's CLS attention."""
     for B, heads, T, hd, causal in ((8, 16, 77, 64, 1), (8, 16, 257, 80, 0)):
         Cw = heads * hd
-        qkv = _addr(1)
+        qkv = addr(1)
         d = sa_desc(B, heads, T, T, hd, causal=causal, q=qkv, k=qkv + 2 * Cw, v=qkv + 4 * Cw, qp=3 * Cw, kp=3 * Cw, vp=3 * Cw,
                     qbs=T * 3 * Cw, kbs=T * 3 * Cw, vbs=T * 3 * Cw)
         assert sa_query(d)[0] is not None
@@ -385,7 +352,7 @@ def test_cls_checker_teeth(T):
     heads, hd = 2, 80
     q, k, v = make_qkv(g, 1, T, heads, hd, "late")
     kv = torch.cat([k, v], dim=1)
-    o, sv = _attn_ref(q.double(), k.double(), v.double(), heads, hd, hd ** -0.5)
+    o, sv = attn_ref(q.double(), k.double(), v.double(), heads, hd, hd ** -0.5)
     bound = attn_expect(o, sv, T, u_p=2.0 ** -22)
     assert float(ratio(emulate_cls(q, kv, heads, hd, hd ** -0.5), o, bound).max()) <= 1.0
     if T > 128:
@@ -393,8 +360,6 @@ def test_cls_checker_teeth(T):
 
 
 # ================================================================================================================ GPU: attention_small
-def _sms(dev):
-    return torch.cuda.get_device_properties(dev).multi_processor_count
 
 
 def sa_layout(B, heads, nq, nkv, hd, causal=0, fused=False):
@@ -434,12 +399,12 @@ def _query_bufs(f, bufs, out_ptr, sms):
 def run_small(R, f, dist="randn", fused=False, expect=None):
     """One GPU case: assert the plan at 132 SMs (and that it is what runs on a 132-SM device), then the census checks; -> worst."""
     bufs = sa_inputs(R, f, dist, fused)
-    plan, err = _query_bufs(f, bufs, _addr(9), SMS)
+    plan, err = _query_bufs(f, bufs, addr(9), SMS)
     assert plan is not None, err
     if expect:
         assert {k: plan[k] for k in expect} == expect, f"plan at 132 SMs {plan}, expected {expect}"
-    if _sms(R.dev) == SMS:
-        assert _query_bufs(f, bufs, _addr(9), 0)[0] == plan
+    if sms(R.dev) == SMS:
+        assert _query_bufs(f, bufs, addr(9), 0)[0] == plan
     errs, (worst, where) = check_attention_small(R, f, bufs)
     assert not errs, f"{errs}; plan {plan}"
     return worst, where, plan
@@ -538,7 +503,7 @@ def test_cls_attention_schedule(cuda, name, shape, dist):
     f = dict(batch=B, tokens=T, heads=heads, hd=hd, qp=Cw + 6, kvp=2 * Cw + 10, op=Cw + 4)
     R = Replay(cuda, zlib.crc32(name.encode()) & 0xFFFF)
     q0, kv = cls_inputs(R, f, dist)
-    plan, err = cls_query(cls_desc(B, T, heads, hd, q=q0.data_ptr(), qp=f["qp"], kv=kv.data_ptr(), kvp=f["kvp"], out=_addr(9), op=f["op"]))
+    plan, err = cls_query(cls_desc(B, T, heads, hd, q=q0.data_ptr(), qp=f["qp"], kv=kv.data_ptr(), kvp=f["kvp"], out=addr(9), op=f["op"]))
     assert plan is not None and plan["smem_bytes"] == (hd + T) * 4, err
     errs, (worst, where) = check_cls(R, f, q0, kv, hd ** -0.5)
     assert not errs, errs
@@ -546,8 +511,6 @@ def test_cls_attention_schedule(cuda, name, shape, dist):
 
 
 # ================================================================================================================ GPU: placement
-def _launches():
-    return _lib().load().ladi_launch_count()
 
 
 SA_GPU_REJECT = [("k misaligned", dict(k=8)), ("v misaligned", dict(v=4)), ("q misaligned", dict(q=2)), ("out misaligned", dict(out=2)),
@@ -561,7 +524,7 @@ SA_GPU_REJECT = [("k misaligned", dict(k=8)), ("v misaligned", dict(v=4)), ("q m
 def test_attention_small_placement_rejected_on_device(cuda, name, delta):
     """The query rejects first; then the launching call returns the same error, launches nothing and leaves the output NaN.  Every
     pointer is an offset view into a valid allocation."""
-    L = _lib().load()
+    L = ladi_lib().load()
     R = Replay(cuda, 7)
     f = sa_layout(2, 2, 20, 365, 128)
     bufs = sa_inputs(R, f, "randn", False)
@@ -572,11 +535,11 @@ def test_attention_small_placement_rejected_on_device(cuda, name, delta):
         a[k] += dv
     plan, err = sa_query(a, 0)
     assert plan is None and err, plan
-    before = _launches()
+    before = launches()
     assert L.ladi_attention_small(*[a[k] for k in SA_ORDER], None) == 1
     assert L.ladi_last_error().decode() == err
     torch.cuda.synchronize()
-    assert _launches() == before
+    assert launches() == before
     assert bool(torch.isnan(out.float()).all())
 
 
@@ -587,7 +550,7 @@ CLS_GPU_REJECT = [("kv misaligned", dict(kv=2)), ("kv_pitch below 2 heads hd", d
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,delta", CLS_GPU_REJECT, ids=[r[0] for r in CLS_GPU_REJECT])
 def test_cls_placement_rejected_on_device(cuda, name, delta):
-    L = _lib().load()
+    L = ladi_lib().load()
     R = Replay(cuda, 8)
     B, T, heads, hd = 1, 12204, 1, 80
     f = dict(batch=B, tokens=T, heads=heads, hd=hd, qp=hd + 6, kvp=2 * hd + 10, op=hd + 4)
@@ -599,9 +562,9 @@ def test_cls_placement_rejected_on_device(cuda, name, delta):
         a[k] += dv
     plan, err = cls_query(a)
     assert plan is None and err, plan
-    before = _launches()
+    before = launches()
     assert L.ladi_cls_attention(*[a[k] for k in CLS_ORDER], None) == 1
     assert L.ladi_last_error().decode() == err
     torch.cuda.synchronize()
-    assert _launches() == before
+    assert launches() == before
     assert bool(torch.isnan(out.float()).all())

@@ -10,12 +10,10 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from kernel_check import rel_l2
+from model_pairs import tps_pair, unet_pair
+
 pytestmark = pytest.mark.gpu
-
-
-def rel_l2(y, ref):
-    y, ref = y.detach().float().cpu(), ref.detach().float().cpu()
-    return ((y - ref).norm() / ref.norm().clamp_min(1e-12)).item()
 
 
 def nhwc(x):
@@ -107,31 +105,9 @@ def test_conv4x4_stride2_through_space_to_depth(cuda):
     assert rel_l2(y, nhwc(ref)) < 1e-2
 
 
-def _tps_pair(cuda):
-    from ladi_oracle import warp as ow
-    from ladi_vton_b200 import synthetic as S
-    from ladi_vton_b200.warp import ConvNet_TPS, control_points
-    eng = ConvNet_TPS(256, 192, 21, 3)
-    sd = S.warp_state_dict(eng.param_shapes(), 11, ctrl_bias=torch.atanh(control_points()).view(-1))
-    o = ow.ConvNet_TPS(256, 192, 21, 3).eval()
-    o.load_state_dict(sd, strict=False)
-    return eng.load_state_dict(sd).to(cuda), o
-
-
-def _unet_pair(cuda, widths=(64, 128, 256, 512, 1024)):
-    from ladi_oracle import warp as ow
-    from ladi_vton_b200 import synthetic as S
-    from ladi_vton_b200.warp import UNetVanilla
-    eng = UNetVanilla(24, 3, True, widths=widths)
-    sd = S.warp_state_dict(eng.param_shapes(), 12)
-    o = ow.UNetVanilla(24, 3, True, widths=widths).eval()
-    o.load_state_dict(sd)
-    return eng.load_state_dict(sd).to(cuda), o
-
-
 def test_convnet_tps(cuda):
     """hubconf.py:57 configuration: ConvNet_TPS(256, 192, 21, 3) -> 25 control points and the [256, 192] sampling grid."""
-    eng, o = _tps_pair(cuda)
+    eng, o = tps_pair(cuda)
     g = torch.Generator().manual_seed(5)
     a, b = torch.rand((2, 3, 256, 192), generator=g) * 2 - 1, torch.rand((2, 21, 256, 192), generator=g)
     with torch.no_grad():
@@ -148,7 +124,7 @@ def test_convnet_tps(cuda):
 
 @pytest.mark.parametrize("widths,hw", [((16, 32, 64, 128, 256), (64, 48)), ((64, 128, 256, 512, 1024), (64, 48))])
 def test_unet_vanilla(cuda, widths, hw):
-    eng, o = _unet_pair(cuda, widths)
+    eng, o = unet_pair(cuda, widths)
     x = torch.rand((2, 24, *hw), generator=torch.Generator().manual_seed(6)) * 2 - 1
     with torch.no_grad():
         ref = o(x)
@@ -164,8 +140,8 @@ def test_generate_warped_cloth_full_size(cuda):
     """src/inference.py:236-263 at 512x384: resizes, TPS, grid_sample, refinement, clamp."""
     from ladi_oracle import warp as ow
     from ladi_vton_b200 import generate_warped_cloth, ops, synthetic as S
-    tps, otps = _tps_pair(cuda)
-    ref_net, oref = _unet_pair(cuda)
+    tps, otps = tps_pair(cuda)
+    ref_net, oref = unet_pair(cuda)
     inp = S.warp_inputs(1, 512, 384, seed=7)
     with torch.no_grad():
         want, coarse, low_grid, pts = ow.warp_cloth(otps, oref, inp["cloth"], inp["im_mask"], inp["pose_map"], return_all=True)
