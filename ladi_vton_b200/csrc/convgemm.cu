@@ -179,9 +179,15 @@ __device__ __forceinline__ float2 ln_fold_row(const KParams& p, const TileRow& r
 // Staged epilogue: the BM x BN bf16 tile goes through shared memory and leaves as whole 16-byte chunks per output row.
 // Staging layout: row r (of the 128 tile rows) is BN * 2 bytes; its 16-byte chunk c sits at chunk c ^ f(r), so that the 8 rows a
 // stmatrix / ldmatrix matrix addresses, and the 8 consecutive chunks a quarter-warp drains, hit 8 distinct bank groups.
+// BN = 32 (64-byte rows, two per 128-byte bank window) and BN = 160 (320-byte rows: 20 chunks, odd rows start half a bank window in)
+// XOR the low 2 bits with the row pair, which keeps a chunk inside its aligned 4-chunk group and so inside the row (c ^ (r & 7) would
+// move chunks 16-19 of a 160-wide row past its end).  At BN = 160 the odd rows' half-window offset turns that into 8 distinct bank
+// groups for any 8 consecutive rows, and a drain phase that crosses from a row's last 4 chunks into the next row's first 4 finds them
+// in opposite halves of the window.  Bank conflicts per 128-row tile at BN = 160 (extra shared-memory wavefronts / access phases):
+// stmatrix / ldmatrix 0 / 320, GEGLU b16 stores 0 / 320, residual fill 0 / 320, drain 0 / 320, GEGLU drain (10-chunk rows) 96 / 160.
 template <int BN>
 __device__ __forceinline__ uint32_t stage_off(int r, int c) {
-  const int pc = BN >= 64 ? (c ^ (r & 7)) : (c ^ ((r >> 1) & 3));  // BN = 32: 64-byte rows, two per 128-byte bank window
+  const int pc = (BN == 32 || BN == 160) ? (c ^ ((r >> 1) & 3)) : (c ^ (r & 7));
   return (uint32_t)(r * (BN * 2) + pc * 16);
 }
 constexpr int STAGE_ROWTAB_BYTES = BM * 8;  // per tile row: output pixel index, or -1 past the extent
@@ -346,7 +352,9 @@ convgemm_kernel(const __grid_constant__ AMaps amaps, const __grid_constant__ CUt
     if (warp == 0) {
       // ------------------------------------------------------------------ TMA producer (warp-uniform loop, one elected lane issues)
       uint32_t stage = 0, phase = 0;
-      for (int item = worker; item < num_items; item += nworkers) {
+      // single CTA: blockIdx.x / gridDim.x read where they are used (not `worker` held from the prologue) keep ptxas from spilling the
+      // item counter of convgemm_kernel<160, false>
+      for (int item = PAIR ? worker : (int)blockIdx.x; item < num_items; item += PAIR ? nworkers : (int)gridDim.x) {
         const int tile = item_tile(item), split = PAIR ? 0 : item - tile * p.splits;
         const int kb0 = split * p.kb_per_split, kb1 = min(p.total_kb, kb0 + p.kb_per_split);
         const TileCoord tc = tile_coord(p, tile);
@@ -392,7 +400,7 @@ convgemm_kernel(const __grid_constant__ AMaps amaps, const __grid_constant__ CUt
     const int rbase = 64 * cw + 16 * (warp & 3) + (lane >> 2);  // this thread's rows: rbase and rbase + 8
     uint32_t stage = 0, phase = 0;
     float acc[BN / 2];
-    for (int item = worker; item < num_items; item += nworkers) {
+    for (int item = PAIR ? worker : (int)blockIdx.x; item < num_items; item += PAIR ? nworkers : (int)gridDim.x) {
       const int tile = item_tile(item), split = PAIR ? 0 : item - tile * p.splits;
       const int nkb = min(p.total_kb, (split + 1) * p.kb_per_split) - split * p.kb_per_split;
       uint32_t prev = 0;
@@ -427,7 +435,7 @@ convgemm_kernel(const __grid_constant__ AMaps amaps, const __grid_constant__ CUt
         rbias[h] = (p.bias_per_row && bias != nullptr && row[h].ok) ? bias[row[h].grow] : 0.f;
       }
       // ---------------------------------------------------------------- staged: row table, then the body of the launch's form
-      if constexpr (!PAIR && BN <= 128) {
+      if constexpr (!PAIR && (BN <= 128 || BN == 160)) {
         if (p.staged) {
           ptx::named_barrier_sync(1 + cw, 128);  // the previous tile's drain has read the staging tile and the row table
           if (q == 0) {
@@ -792,17 +800,32 @@ Plan choose_plan(const ladi_conv_desc* d, int tiles_m, int total_kb, int sms) {
       }
     }
   }
-  // 3. else minimise (waves x per-tile cost) with per-tile cost ~ BN + fixed A-operand cost.  Tiles wider than 128 (160-256, still
-  // available through force_bn) made the default workload slower on H100 (2850 vs 2450 ms per call, 512x384, batch 8, CFG, 400 W card;
-  // 160 alone as an automatic candidate: 2602 vs 2455 ms).
+  // ---- store path, as far as the descriptor decides it: bf16 rows of whole, aligned 16-byte chunks can be staged through shared memory
+  // (16-byte stores); fp32 / split-K partials, the LayerNorm fold, row statistics and odd widths take fragment stores
+  const int out_cols = d->act == 2 ? d->c_out / 2 : d->c_out;
+  const bool col_bias = d->bias != nullptr && !d->bias_per_row;
+  const bool stageable = !d->out_fp32 && d->rowstat_out == nullptr && d->ln_stats == nullptr &&
+                         out_cols % 8 == 0 && d->c_out % 8 == 0 && d->out_pitch % 8 == 0 && reinterpret_cast<uintptr_t>(d->out) % 16 == 0 &&
+                         (d->residual == nullptr || (d->residual_pitch % 8 == 0 && reinterpret_cast<uintptr_t>(d->residual) % 16 == 0)) &&
+                         (!col_bias || (reinterpret_cast<uintptr_t>(d->bias) % 8 == 0 && d->bias_step_stride % 2 == 0));
+  const bool pairs = d->pair_mode == 1 || (d->pair_mode == 0 && ladi_conv_pair_default());
+  // 3. else minimise (waves x per-tile cost), per-tile cost ~ BN + fixed A-operand cost for 128 / 64 / 32.  160 is a candidate only for
+  // a long reduction (total_kb > 8) that takes the staged epilogue: short reductions keep the full-width 128 tile (below), and 160 with
+  // fragment stores made the default workload slower (2602 vs 2455 ms per call, 512x384, batch 8, CFG, H100 at 400 W; measured before
+  // the staged epilogue existed, when every launch stored from the fragment).  Its per-tile cost, 240, is 1.25 x the 128 tile's: what
+  // tools/sweep_conv_tiles.py measured for long-K launches of the UNet step whose waves 160 does not cut (H100 80GB HBM3, 700 W).  So 160
+  // wins where it removes a padded tile (c_out 320) or enough waves (c_out 640 at 96 M tiles: 4 -> 3); a tie keeps the old tile, which
+  // leaves alone the launches the sweep showed no better or slower at 160 (c_out 1920, 3840, 5120 and 10240 at 24 or 96 M tiles).
+  // 192 / 256 stay available through force_bn.
   if (pl.bn == 0) {
-    static const int cand[3] = {128, 64, 32};
+    static const int cand[4] = {128, 64, 32, 160};  // 160 last: a tie keeps the narrower tile
     long best = -1;
-    for (int i = 0; i < 3; ++i) {
+    for (int i = 0; i < 4; ++i) {
       if (d->pair_mode == 1 && cand[i] < 128) continue;  // forced CTA pairs need a tile they can split
       if (total_kb <= 8 && d->c_out >= 128 && cand[i] < 128) continue;  // short reductions (K <= 512): the full-width tile
+      if (cand[i] == 160 && !(total_kb > 8 && d->c_out >= 160 && stageable && !pairs)) continue;
       const long tiles = (long)tiles_m * ((d->c_out + cand[i] - 1) / cand[i]);
-      const long cost = ((tiles + sms - 1) / sms) * (cand[i] + 64);
+      const long cost = ((tiles + sms - 1) / sms) * (cand[i] == 160 ? 240 : cand[i] + 64);
       if (best < 0 || cost < best) { best = cost; pl.bn = cand[i]; }
     }
   }
@@ -816,14 +839,9 @@ Plan choose_plan(const ladi_conv_desc* d, int tiles_m, int total_kb, int sms) {
     // default: pair whenever there are enough M tiles that the phantom tile of an odd count is noise
     else if (d->pair_mode == 0 && ladi_conv_pair_default()) pl.pair = tiles_m >= 4 && (tiles_m % 2 == 0 || tiles_m >= 16);
   }
-  // ---- epilogue: staged through shared memory (16-byte stores) for bf16 rows of whole, aligned 16-byte chunks; fragment stores for
-  // fp32 / split-K partials, the LayerNorm fold and row statistics, odd widths, CTA pairs and N tiles wider than 128
-  const int out_cols = d->act == 2 ? d->c_out / 2 : d->c_out;
-  const bool col_bias = d->bias != nullptr && !d->bias_per_row;
-  pl.staged = !pl.pair && !split && pl.bn <= 128 && !d->out_fp32 && d->rowstat_out == nullptr && d->ln_stats == nullptr &&
-              out_cols % 8 == 0 && d->c_out % 8 == 0 && d->out_pitch % 8 == 0 && reinterpret_cast<uintptr_t>(d->out) % 16 == 0 &&
-              (d->residual == nullptr || (d->residual_pitch % 8 == 0 && reinterpret_cast<uintptr_t>(d->residual) % 16 == 0)) &&
-              (!col_bias || (reinterpret_cast<uintptr_t>(d->bias) % 8 == 0 && d->bias_step_stride % 2 == 0));
+  // ---- epilogue: staged for the tiles staged_dispatch is instantiated for (160 only past the short-reduction rule); CTA pairs and split-K
+  // partials store from the fragment
+  pl.staged = stageable && !pl.pair && !split && (pl.bn <= 128 || (pl.bn == 160 && total_kb > 8));
   pl.form = d->act | (d->residual != nullptr ? 1 << 3 : 0) | (col_bias ? 1 << 4 : 0);
   return pl;
 }
