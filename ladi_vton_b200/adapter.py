@@ -13,10 +13,11 @@ import torch
 
 from . import engine as eng, lib, ops
 from .clip import encoder_layer, encoder_layer_shapes, pack_encoder_layer
+from .module import PackedModule
 from .weights import f32, pack_linear
 
 
-class InversionAdapter:
+class InversionAdapter(PackedModule):
     def __init__(self, input_dim=1280, hidden_dim=5120, output_dim=16384, config=None, num_encoder_layers=1, dropout=0.5, heads=16, mlp_dim=5120):
         if config is not None:  # accept the reference's `config=config.vision_config`
             heads = getattr(config, "num_attention_heads", heads)
@@ -25,14 +26,6 @@ class InversionAdapter:
             raise ValueError(f"num_encoder_layers must be >= 1, got {num_encoder_layers}")
         self.num_encoder_layers = int(num_encoder_layers)
         self.dim, self.hidden, self.out_dim, self.heads, self.mlp_dim = input_dim, hidden_dim, output_dim, heads, mlp_dim
-        self.device = torch.device("cpu")
-        self._sd, self.P = None, None
-
-    def eval(self):
-        return self
-
-    def requires_grad_(self, flag=False):
-        return self
 
     def param_shapes(self):
         d, S = self.dim, {}
@@ -44,29 +37,7 @@ class InversionAdapter:
         S["layers.6.weight"], S["layers.6.bias"] = (self.out_dim, self.hidden), (self.out_dim,)
         return S
 
-    def load_state_dict(self, sd, strict=True):
-        want = self.param_shapes()
-        bad = [k for k in want if k not in sd or tuple(sd[k].shape) != tuple(want[k])] + [k for k in sd if k not in want]
-        if strict and bad:
-            raise RuntimeError(f"InversionAdapter state_dict mismatch: {bad[:6]}")
-        self._sd = {k: v.detach() for k, v in sd.items()}
-        if self.device.type == "cuda":
-            self._pack()
-        return self
-
-    def to(self, device=None, dtype=None, **kw):
-        if isinstance(device, torch.dtype):
-            device = None
-        if device is not None:
-            device = torch.device(device)
-            if device.type != "cuda":
-                raise RuntimeError("ladi_vton_b200 InversionAdapter runs on CUDA (sm_90a) only; there is no CPU path")
-            self.device = device
-            if self._sd is not None:
-                self._pack()
-        return self
-
-    def _pack(self):
+    def _pack_weights(self):
         g = lambda k: self._sd[k].to(self.device, torch.float32)
         L = self.num_encoder_layers
         e = f"encoder_layers.{L - 1}."
@@ -82,10 +53,10 @@ class InversionAdapter:
                      ("l0", "layers.0"), ("l3", "layers.3"), ("l6", "layers.6")):
             P[n + ".w"], P[n + ".b"] = pack_linear(g(k + ".weight")), f32(g(k + ".bias"))
         self.P = P
-        self.engine = None
-        if eng.enabled() and self.device.type == "cuda":
-            self.engine = eng.Engine(eng.flatten(P, "adapter."), adapter_dim=self.dim, adapter_heads=self.heads, adapter_mlp=self.mlp_dim,
-                                     adapter_hidden=self.hidden, adapter_out=self.out_dim)
+
+    def _make_engine(self):
+        return eng.Engine(eng.flatten(self.P, "adapter."), adapter_dim=self.dim, adapter_heads=self.heads, adapter_mlp=self.mlp_dim,
+                          adapter_hidden=self.hidden, adapter_out=self.out_dim)
 
     def __call__(self, x):
         """x [B, 257, 1280] (CLIP vision last_hidden_state, any float dtype) -> [B, 16384] bf16."""
@@ -93,7 +64,7 @@ class InversionAdapter:
         B, T, _ = x.shape
         hd = d // self.heads
         xb = x.to(self.device, torch.bfloat16).contiguous()
-        if getattr(self, "engine", None) is not None and ops.PROFILE is None and lib.RECORD is None:  # one ABI call (csrc/engine.cu adapter_forward)
+        if self.use_engine():  # one ABI call (csrc/engine.cu adapter_forward)
             out = torch.empty((B, self.out_dim), dtype=torch.bfloat16, device=self.device)
             ws = self.engine.workspace(eng.MODULE_ADAPTER, B, T, 0)
             lib.call("ladi_inversion_adapter_forward", self.engine.h, ops._ptr(xb), B, T, ops._ptr(out), ops._ptr(ws), ws.numel(), ops._stream())

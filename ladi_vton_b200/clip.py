@@ -17,17 +17,10 @@ the wgmma kernel of the hot path (fused QKV, GELU / residual epilogues), LayerNo
 import torch
 
 from . import ops
+from .module import PackedModule, _Cfg
 from .weights import f32, pack_linear
 
 DOLLAR_ID = 259  # '$' (encode_text_word_embedding.py:13)
-
-
-class _Cfg(dict):
-    def __getattr__(self, k):
-        try:
-            return self[k]
-        except KeyError:
-            raise AttributeError(k)
 
 
 class CLIPOutput:
@@ -42,47 +35,16 @@ class CLIPOutput:
         return (self.last_hidden_state, self.pooler_output)[i]
 
 
-class _Tower:
-    """Shared: device handling, layer packing, the pre-LN transformer stack."""
+class _Tower(PackedModule):
+    """Shared: layer packing, the pre-LN transformer stack."""
     prefix = ""
 
     def __init__(self, **config):
         self.config = _Cfg(config)
-        self.device = torch.device("cpu")
         self.dtype = torch.bfloat16
-        self._sd, self.P = None, None
 
-    def eval(self):
-        return self
-
-    def requires_grad_(self, flag=False):
-        return self
-
-    def param_shapes(self):
-        raise NotImplementedError
-
-    def load_state_dict(self, sd, strict=True):
-        want = self.param_shapes()
-        ignore = lambda k: k.endswith("position_ids") or k.startswith("visual_projection") or k.startswith("text_projection")
-        bad = [k for k in want if k not in sd or tuple(sd[k].shape) != tuple(want[k])] + [k for k in sd if k not in want and not ignore(k)]
-        if strict and bad:
-            raise RuntimeError(f"{type(self).__name__} state_dict mismatch: {bad[:6]}")
-        self._sd = {k: v.detach() for k, v in sd.items() if k in want}
-        if self.device.type == "cuda":
-            self._pack()
-        return self
-
-    def to(self, device=None, dtype=None, **kw):
-        if isinstance(device, torch.dtype):
-            device = None
-        if device is not None:
-            device = torch.device(device)
-            if device.type != "cuda":
-                raise RuntimeError(f"ladi_vton_b200 {type(self).__name__} runs on CUDA (sm_90a) only; there is no CPU path")
-            self.device = device
-            if self._sd is not None:
-                self._pack()
-        return self
+    def ignorable(self, key):  # transformers checkpoints also hold these; the path here never reads them
+        return key.endswith("position_ids") or key.startswith(("visual_projection", "text_projection"))
 
     def _pack_layers(self, P):
         g = lambda k: self._sd[k].to(self.device, torch.float32)
@@ -156,7 +118,7 @@ class CLIPTextModel(_Tower):
         S["text_model.final_layer_norm.weight"], S["text_model.final_layer_norm.bias"] = (d,), (d,)
         return S
 
-    def _pack(self):
+    def _pack_weights(self):
         g = lambda k: self._sd[k].to(self.device, torch.float32)
         P = {}
         P["tok"] = g("text_model.embeddings.token_embedding.weight").to(torch.bfloat16).contiguous()
@@ -235,7 +197,7 @@ class CLIPVisionModelWithProjection(_Tower):
             encoder_layer_shapes(S, f"vision_model.encoder.layers.{i}.", d, c.intermediate_size)
         return S
 
-    def _pack(self):
+    def _pack_weights(self):
         g = lambda k: self._sd[k].to(self.device, torch.float32)
         P = {}
         P["cls"] = g("vision_model.embeddings.class_embedding").to(torch.bfloat16).contiguous()

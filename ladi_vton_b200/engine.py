@@ -3,7 +3,8 @@ weights, and the per-module entry points -- `ladi_unet_forward`, `ladi_vae_encod
 `ladi_inversion_adapter_forward`, `ladi_denoise_loop` -- the launch sequences of which live in C++.  The Python model classes
 (unet.py / vae.py / adapter.py) are thin callers of these; their own Python sequencing of the same kernels is kept for two purposes only:
 per-launch instrumentation (ops.PROFILE, bench.py's roofline pass) and the CPU test that pins the C++ sequence to it op by op
-(tests/test_engine_trace.py).  Env LADI_ENGINE=0 forces the Python sequencing (A/B).
+(tests/test_engine_trace.py).  Env LADI_ENGINE=0 forces the Python sequencing (A/B).  When a model builds its handle and when a call
+takes it is decided in one place, module.PackedModule (`_pack`, `use_engine`).
 """
 import ctypes as C
 import os

@@ -25,6 +25,7 @@ import numpy as np
 import torch
 
 from . import lib, ops
+from .module import PackedModule
 from .weights import pad64
 
 INCEPTION_BN_EPS = 1e-3
@@ -160,50 +161,8 @@ class _Conv:
         return out
 
 
-class _Net:
-    def __init__(self):
-        self.device = torch.device("cpu")
-        self._sd = None
-        self.layers = None
-
-    def eval(self):
-        return self
-
-    def requires_grad_(self, flag=False):
-        return self
-
-    def param_shapes(self):
-        raise NotImplementedError
-
-    def load_state_dict(self, sd, strict=True):
-        want = self.param_shapes()
-        missing = [k for k in want if k not in sd or tuple(sd[k].shape) != tuple(want[k])]
-        if strict:
-            extra = [k for k in sd if k not in want and not self._ignorable(k)]
-            if missing or extra:
-                raise RuntimeError(f"{type(self).__name__} state_dict mismatch: missing/misshaped {missing[:6]}, unexpected {extra[:6]}")
-        elif missing:
-            raise RuntimeError(f"{type(self).__name__} state_dict lacks {missing[:6]}")
-        self._sd = {k: sd[k].detach().cpu() for k in want}
-        if self.device.type == "cuda":
-            self._pack()
-        return self
-
-    @staticmethod
-    def _ignorable(k):
-        return False
-
-    def to(self, device=None, dtype=None, **kw):
-        if isinstance(device, torch.dtype):
-            device = None
-        if device is not None:
-            device = torch.device(device)
-            if device.type != "cuda":
-                raise RuntimeError(f"ladi_vton_b200 {type(self).__name__} runs on CUDA (sm_90a) only; there is no CPU path")
-            self.device = device
-            if self._sd is not None:
-                self._pack()
-        return self
+class _Net(PackedModule):
+    layers = None
 
     def _check_ready(self):
         if self.layers is None:
@@ -221,14 +180,14 @@ class FIDInceptionV3(_Net):
         S["fc.weight"], S["fc.bias"] = (1008, 2048), (1008,)
         return S
 
-    def _pack(self):
+    def _pack_weights(self):
         sd, dev = self._sd, self.device
         self.layers = {}
         for name, (_, _, _, s, p) in INCEPTION_LAYERS.items():
             w, b = fold_bn(sd[f"{name}.conv.weight"], sd[f"{name}.bn.weight"], sd[f"{name}.bn.bias"], sd[f"{name}.bn.running_mean"],
                            sd[f"{name}.bn.running_var"], INCEPTION_BN_EPS)
             self.layers[name] = _Conv(w, b, s, p, dev)
-        self.fc_weight = sd["fc.weight"].double()
+        self.fc_weight = sd["fc.weight"].double().cpu()
         self.shift = torch.full((3,), 128.0, device=dev)
         self.scale = torch.full((3,), 128.0, device=dev)
 
@@ -335,11 +294,10 @@ class LPIPSAlex(_Net):
             S[f"lin{t}.model.1.weight"] = (1, c, 1, 1)
         return S
 
-    @staticmethod
-    def _ignorable(k):
-        return k.startswith("classifier.")  # torchvision's AlexNet file also holds the classifier
+    def ignorable(self, key):
+        return key.startswith("classifier.")  # torchvision's AlexNet file also holds the classifier
 
-    def _pack(self):
+    def _pack_weights(self):
         sd, dev = self._sd, self.device
         self.layers = {i: _Conv(sd[f"features.{i}.weight"].double(), sd[f"features.{i}.bias"].double(), s, p, dev)
                        for i, (_, _, _, s, p) in ALEX_LAYERS.items()}

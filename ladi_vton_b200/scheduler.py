@@ -7,14 +7,7 @@ import numpy as np
 import torch
 
 from . import ops
-
-
-class _C(dict):
-    def __getattr__(self, k):
-        try:
-            return self[k]
-        except KeyError as e:
-            raise AttributeError(k) from e
+from .module import _Cfg
 
 
 class _Step:
@@ -30,7 +23,7 @@ class DDIMScheduler:
                  steps_offset=1, clip_sample=False, set_alpha_to_one=False, prediction_type="epsilon", **unused):
         if beta_schedule != "scaled_linear" or prediction_type != "epsilon" or clip_sample:
             raise NotImplementedError("only the SD-2-inpainting DDIM config (scaled_linear, epsilon, clip_sample=False)")
-        self.config = _C(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
+        self.config = _Cfg(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
                          beta_schedule=beta_schedule, steps_offset=steps_offset, clip_sample=clip_sample,
                          set_alpha_to_one=set_alpha_to_one, prediction_type=prediction_type, skip_prk_steps=True)
         betas = torch.linspace(beta_start ** 0.5, beta_end ** 0.5, num_train_timesteps, dtype=torch.float32) ** 2

@@ -23,6 +23,7 @@ import os
 import torch
 
 from . import engine as eng, lib, ops
+from .module import PackedModule, _Cfg
 from .weights import f32, fold_layernorm, interleave_geglu, pack_conv, pack_conv_up2x, pack_linear
 
 LN_EPS = 1e-5  # nn.LayerNorm default (BasicTransformerBlock.norm1/2/3)
@@ -34,14 +35,6 @@ SD2_INPAINT_UNET = dict(
     up_block_types=("UpBlock2D", "CrossAttnUpBlock2D", "CrossAttnUpBlock2D", "CrossAttnUpBlock2D"),
     sample_size=64,
 )
-
-
-class _Cfg(dict):
-    def __getattr__(self, k):
-        try:
-            return self[k]
-        except KeyError as e:
-            raise AttributeError(k) from e
 
 
 class _Sample:
@@ -115,56 +108,20 @@ def unet_param_shapes(cfg):
     return S
 
 
-class UNet2DConditionModel:
+class UNet2DConditionModel(PackedModule):
     def __init__(self, **config):
         self.config = _Cfg({**SD2_INPAINT_UNET, **config})
         self.dtype = torch.bfloat16
-        self.device = torch.device("cpu")
-        self._sd = None
-        self.P = None
         self._steps = None
         self._steps_key = None
         self._ctx = None
-        self.pack_gen = 0  # bumped by every re-pack: captured graphs hold the packed weights' addresses (pipeline._graph_key)
 
     # ---- reference-compatible surface -------------------------------------------------------------------------------
-    def eval(self):
-        return self
-
-    def requires_grad_(self, flag=False):
-        return self
-
     def enable_xformers_memory_efficient_attention(self):  # inference.py:143-147: accepted, attention is already fused
         return self
 
-    def load_state_dict(self, sd, strict=True):
-        shapes = unet_param_shapes(self.config)
-        missing = [k for k in shapes if k not in sd]
-        unexpected = [k for k in sd if k not in shapes]
-        bad = [k for k in shapes if k in sd and tuple(sd[k].shape) != tuple(shapes[k])]
-        if strict and (missing or unexpected or bad):
-            raise RuntimeError(f"UNet state_dict mismatch: missing={missing[:4]} unexpected={unexpected[:4]} shape={bad[:4]}")
-        self._sd = {k: v.detach() for k, v in sd.items()}
-        self.P = None
-        if self.device.type == "cuda":
-            self._pack()
-        return self
-
-    def to(self, device=None, dtype=None, **kw):
-        if isinstance(device, torch.dtype):
-            device, dtype = None, device
-        if device is not None:
-            device = torch.device(device)
-            if device.type != "cuda":
-                raise RuntimeError("ladi_vton_b200 UNet runs on CUDA (sm_90a) only; there is no CPU path")
-            if self.P is not None and device == self.device:
-                return self  # already packed on this device: re-packing would free weights a captured graph still points at
-            self.device = device
-            if self._sd is not None:
-                self._pack()
-            elif self.P is not None:
-                raise RuntimeError("the state dict was released after packing; call load_state_dict again to move the UNet")
-        return self
+    def param_shapes(self):
+        return unet_param_shapes(self.config)
 
     def __call__(self, sample, timestep, encoder_hidden_states, return_dict=True):
         """Generic entry: NCHW sample (any float dtype), scalar timestep, ctx [B,77,ctx_dim]."""
@@ -180,7 +137,7 @@ class UNet2DConditionModel:
         return _Sample(out) if return_dict else (out,)
 
     # ---- packing ------------------------------------------------------------------------------------------------------
-    def _pack(self):
+    def _pack_weights(self):
         sd, dev, cfg = self._sd, self.device, self.config
         g = lambda k: sd[k].to(dev, torch.float32)
         P = {}
@@ -281,13 +238,10 @@ class UNet2DConditionModel:
         self.kv_total = off
         self.P = P
         self.ws = ops.GroupNormWS(dev)
-        self.pack_gen += 1
         self._steps = self._steps_key = self._ctx = None
-        self.engine = None
-        if eng.enabled() and not self.fold_ln and dev.type == "cuda":  # the C++ launch sequence (csrc/engine.cu); LADI_ENGINE=0 -> Python sequencing
-            self.engine = eng.Engine(eng.flatten(P), **self.engine_config())
-        if any(v.is_cuda for v in sd.values()):
-            self._sd = None  # device-resident fp32 source weights (3.5 GB for the full UNet) are not kept beside the bf16 pack
+
+    def _make_engine(self):  # the C++ launch sequence (csrc/engine.cu) has no LayerNorm-folded form
+        return None if self.fold_ln else eng.Engine(eng.flatten(self.P), **self.engine_config())
 
     def engine_config(self):
         cfg = self.config
@@ -305,7 +259,7 @@ class UNet2DConditionModel:
         if self._steps is not None and self._steps_key == key:
             return self._steps  # same schedule as the previous call: the table (and its address) stands
         keep = self._steps if (self._steps is not None and tuple(self._steps.shape) == (len(timesteps), self.temb_total)) else None
-        if getattr(self, "engine", None) is not None and ops.PROFILE is None and lib.RECORD is None:
+        if self.use_engine():
             # one ABI call (csrc/engine.cu unet_plan_steps): sinusoid table on the device, the time MLP and all 22 time_emb_proj as three GEMMs
             n = len(timesteps)
             tdev = torch.tensor([float(x) for x in timesteps], dtype=torch.float32).to(self.device)
@@ -337,7 +291,7 @@ class UNet2DConditionModel:
         c = ctx.to(self.device, torch.bfloat16).contiguous().view(B * T, D)
         if out is None and self._ctx is not None and tuple(self._ctx.shape) == (B, T, self.kv_total):
             out = self._ctx
-        if getattr(self, "engine", None) is not None and ops.PROFILE is None and lib.RECORD is None and D % 8 == 0:
+        if self.use_engine() and D % 8 == 0:
             if out is None:
                 out = torch.empty((B, T, self.kv_total), dtype=torch.bfloat16, device=self.device)
             assert out.is_contiguous()
@@ -399,7 +353,7 @@ class UNet2DConditionModel:
         P, cfg = self.P, self.config
         ch, L, heads = cfg.block_out_channels, cfg.layers_per_block, cfg.attention_head_dim
         assert self._steps is not None and self._ctx is not None, "call plan_steps/plan_context first"
-        if getattr(self, "engine", None) is not None and ops.PROFILE is None and lib.RECORD is None:
+        if self.use_engine():
             # the product path: ONE ABI call, the launch sequence below lives in C++ (csrc/engine.cu unet_forward)
             B, h, w, _ = x_in.shape
             assert x_in.is_contiguous() and x_in.shape[3] == self.in_pitch and self._ctx.is_contiguous() and self._steps.is_contiguous()

@@ -14,7 +14,7 @@ import os
 import torch
 
 from . import engine as eng, lib, ops
-from .unet import _Cfg
+from .module import PackedModule, _Cfg
 from .weights import f32, pack_conv, pack_conv_up2x, pack_linear
 
 SD2_VAE = dict(in_channels=3, out_channels=3, block_out_channels=(128, 256, 512, 512), layers_per_block=2,
@@ -94,50 +94,16 @@ class _Dec:
         self.sample = s
 
 
-class AutoencoderKL:
+class AutoencoderKL(PackedModule):
     def __init__(self, **config):
         self.config = _Cfg({**SD2_VAE, **config})
         self.dtype = torch.bfloat16
-        self.device = torch.device("cpu")
-        self._sd, self.P = None, None
-        self.pack_gen = 0
 
-    def eval(self):
-        return self
-
-    def requires_grad_(self, flag=False):
-        return self
-
-    def load_state_dict(self, sd, strict=True):
-        shapes = vae_param_shapes(self.config)
-        missing = [k for k in shapes if k not in sd]
-        unexpected = [k for k in sd if k not in shapes]
-        bad = [k for k in shapes if k in sd and tuple(sd[k].shape) != tuple(shapes[k])]
-        if strict and (missing or unexpected or bad):
-            raise RuntimeError(f"VAE state_dict mismatch: missing={missing[:4]} unexpected={unexpected[:4]} shape={bad[:4]}")
-        self._sd = {k: v.detach() for k, v in sd.items()}
-        if self.device.type == "cuda":
-            self._pack()
-        return self
-
-    def to(self, device=None, dtype=None, **kw):
-        if isinstance(device, torch.dtype):
-            device = None
-        if device is not None:
-            device = torch.device(device)
-            if device.type != "cuda":
-                raise RuntimeError("ladi_vton_b200 VAE runs on CUDA (sm_90a) only; there is no CPU path")
-            if self.P is not None and device == self.device:
-                return self  # already packed here (captured graphs hold these addresses)
-            self.device = device
-            if self._sd is not None:
-                self._pack()
-            elif self.P is not None:
-                raise RuntimeError("the state dict was released after packing; call load_state_dict again to move the VAE")
-        return self
+    def param_shapes(self):
+        return vae_param_shapes(self.config)
 
     # ------------------------------------------------------------------------------------------------------------------
-    def _pack(self):
+    def _pack_weights(self):
         sd, dev, cfg = self._sd, self.device, self.config
         g = lambda k: sd[k].to(dev, torch.float32)
         P = {}
@@ -198,21 +164,15 @@ class AutoencoderKL:
         norm("decoder.conv_norm_out"); conv("decoder.conv_out", ch[0])
         self.P = P
         self.ws = ops.GroupNormWS(dev)
-        self.pack_gen += 1
-        if any(v.is_cuda for v in sd.values()):
-            self._sd = None
-        self.engine = None
-        if eng.enabled() and dev.type == "cuda":
-            self.engine = eng.Engine(eng.flatten(P), **self.engine_config())
+
+    def _make_engine(self):
+        return eng.Engine(eng.flatten(self.P), **self.engine_config())
 
     def engine_config(self):
         cfg = self.config
         return dict(vae_channels=cfg.block_out_channels, vae_layers_per_block=cfg.layers_per_block, vae_latent_channels=cfg.latent_channels,
                     vae_in_channels=cfg.in_channels, vae_out_channels=cfg.out_channels, norm_groups=cfg.norm_num_groups,
                     fuse_upsample=int(self.fuse_up), emasc_scales=5)
-
-    def _use_engine(self):
-        return getattr(self, "engine", None) is not None and ops.PROFILE is None and lib.RECORD is None
 
     # ------------------------------------------------------------------------------------------------------------------
     def _resnet(self, p, x, co):
@@ -257,7 +217,7 @@ class AutoencoderKL:
             B, _, H, W = x.shape
             xin = torch.zeros((B, H, W, 8), dtype=torch.bfloat16, device=self.device)
             ops.nchw_to_nhwc(x.to(self.device, torch.float32).contiguous(), xin)
-        if self._use_engine():  # one ABI call (csrc/engine.cu vae_encode); the retained features are written into caller buffers
+        if self.use_engine():  # one ABI call (csrc/engine.cu vae_encode); the retained features are written into caller buffers
             mk = lambda c, f: torch.empty((B, H // f, W // f, c), dtype=torch.bfloat16, device=self.device)
             f1, f3, f4, f5 = mk(ch[0], 1), mk(ch[0], 2), mk(ch[1], 4), mk(ch[2], 8)
             mom = torch.empty((B, H // 8, W // 8, 2 * cfg.latent_channels), dtype=torch.float32, device=self.device)
@@ -294,7 +254,7 @@ class AutoencoderKL:
         B, _, h, w = z.shape
         zin = torch.zeros((B, h, w, 8), dtype=torch.bfloat16, device=self.device)
         ops.nchw_to_nhwc(z.to(self.device, torch.float32).contiguous(), zin, scale=scale)
-        if self._use_engine():  # one ABI call (csrc/engine.cu vae_decode)
+        if self.use_engine():  # one ABI call (csrc/engine.cu vae_decode)
             img = torch.empty((B, 8 * h, 8 * w, 4), dtype=torch.float32, device=self.device)
             fl = list(feats) if feats else []
             lay = [int(i) for i in (int_layers or [])][:len(fl)]
@@ -342,7 +302,7 @@ class AutoencoderKL:
         return _Dec(ops.nhwc_to_nchw(img, self.config.out_channels))
 
 
-class EMASC:
+class EMASC(PackedModule):
     """emasc.py:11-40: per scale either the nonlinear form Conv(k) -> SiLU -> Conv(k) (state-dict keys conv.{i}.{0,2}.{weight,bias}; the
     hub checkpoints are k = 3) or the linear form, one Conv3x3 (keys conv.{i}.{weight,bias}; the reference's linear EMASC always builds a
     3x3 kernel and ignores `kernel_size`, emasc.py:21-24).  `mask_features` is folded into the last conv's epilogue."""
@@ -362,45 +322,12 @@ class EMASC:
                 "(csrc/convgemm.cu); only 3x3 and 1x1 EMASC run on it")
         self.type, self.kernel_size, self.padding = type, k, padding
         self.in_channels, self.out_channels = list(in_channels), list(out_channels)
-        self.device = torch.device("cpu")
-        self._sd, self.P = None, None
-        self.pack_gen = 0
-
-    def eval(self):
-        return self
-
-    def requires_grad_(self, flag=False):
-        return self
 
     def param_shapes(self):
         from .synthetic import emasc_param_shapes
         return emasc_param_shapes(self.in_channels, self.out_channels, self.kernel_size, self.type)
 
-    def load_state_dict(self, sd, strict=True):
-        want = self.param_shapes()
-        bad = sorted(set(sd.keys()) ^ set(want)) + [k for k in want if k in sd and tuple(sd[k].shape) != tuple(want[k])]
-        if strict and bad:
-            raise RuntimeError(f"EMASC state_dict mismatch: {bad[:6]}")
-        self._sd = {k: v.detach() for k, v in sd.items()}
-        if self.device.type == "cuda":
-            self._pack()
-        return self
-
-    def to(self, device=None, dtype=None, **kw):
-        if isinstance(device, torch.dtype):
-            device = None
-        if device is not None:
-            device = torch.device(device)
-            if device.type != "cuda":
-                raise RuntimeError("ladi_vton_b200 EMASC runs on CUDA (sm_90a) only; there is no CPU path")
-            if self.P is not None and device == self.device:
-                return self
-            self.device = device
-            if self._sd is not None:
-                self._pack()
-        return self
-
-    def _pack(self):
+    def _pack_weights(self):
         g = lambda k: self._sd[k].to(self.device, torch.float32)
         self.P = []
         for i, ci in enumerate(self.in_channels):
@@ -409,11 +336,10 @@ class EMASC:
             else:  # (w1, b1, w2, b2)
                 self.P.append((pack_conv(g(f"conv.{i}.0.weight"), [ci]), f32(g(f"conv.{i}.0.bias")),
                                pack_conv(g(f"conv.{i}.2.weight"), [ci]), f32(g(f"conv.{i}.2.bias"))))
-        self.pack_gen += 1
-        self.engine = None
-        if eng.enabled() and self.device.type == "cuda":
-            self._engine_weights = self.engine_weights()
-            self.engine = {}  # one handle per resolution pyramid (the strides are part of the handle's config), built on first use
+
+    def _make_engine(self):
+        self._engine_weights = self.engine_weights()
+        return {}  # one handle per resolution pyramid (the strides are part of the handle's config), built on first use
 
     def engine_weights(self):
         """Weight table of ladi_emasc_forward: emasc.<i>.w1/b1 (+ w2/b2 for the nonlinear form; the engine reads the form and the kernel
@@ -435,7 +361,7 @@ class EMASC:
 
     def __call__(self, feats, inv_masks=None):
         """feats: list of NHWC bf16 tensors; inv_masks: optional list of fp32 (1-mask) rows per scale => mask_features fused."""
-        if getattr(self, "engine", None) is not None and ops.PROFILE is None and lib.RECORD is None and len(feats) == len(self.P):
+        if self.use_engine() and len(feats) == len(self.P):
             e, H, Wd = self._engine_for(feats)  # one ABI call (csrc/engine.cu emasc_forward)
             B = feats[0].shape[0]
             outs = []

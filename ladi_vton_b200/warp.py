@@ -19,49 +19,15 @@ import itertools
 import torch
 
 from . import ops
+from .module import PackedModule
 from .weights import f32, pack_conv, pack_linear
 
 BN_EPS = 1e-5
 
 
-class _Module:
-    def __init__(self):
-        self.device = torch.device("cpu")
-        self._sd, self.P = None, None
-
-    def eval(self):
-        return self
-
-    def requires_grad_(self, flag=False):
-        return self
-
-    def param_shapes(self):
-        raise NotImplementedError
-
-    optional_prefixes = ()
-
-    def load_state_dict(self, sd, strict=True):
-        want = self.param_shapes()
-        opt = lambda k: k.endswith("num_batches_tracked") or k.startswith(self.optional_prefixes)
-        bad = [k for k in want if not opt(k) and (k not in sd or tuple(sd[k].shape) != tuple(want[k]))] + [k for k in sd if k not in want]
-        if strict and bad:
-            raise RuntimeError(f"{type(self).__name__} state_dict mismatch: {bad[:6]}")
-        self._sd = {k: v.detach() for k, v in sd.items() if k in want}
-        if self.device.type == "cuda":
-            self._pack()
-        return self
-
-    def to(self, device=None, dtype=None, **kw):
-        if isinstance(device, torch.dtype):
-            device = None
-        if device is not None:
-            device = torch.device(device)
-            if device.type != "cuda":
-                raise RuntimeError(f"ladi_vton_b200 {type(self).__name__} runs on CUDA (sm_90a) only; there is no CPU path")
-            self.device = device
-            if self._sd is not None:
-                self._pack()
-        return self
+class _Module(PackedModule):
+    def optional(self, key):  # BatchNorm's step counter is unused in eval; TPSGridGen's buffers are recomputed when absent (tps_matrices)
+        return key.endswith("num_batches_tracked") or key.startswith("gridGen.")
 
     def _g(self, k):
         return self._sd[k].to(self.device, torch.float32)
@@ -122,10 +88,7 @@ def tps_matrices(height, width, ctrl):
 
 
 class ConvNet_TPS(_Module):
-    optional_prefixes = ("gridGen.",)
-
     def __init__(self, height, width, input_nc=6, n_layer=4):
-        super().__init__()
         f = 2 ** (n_layer + 1)
         if height % (4 * f) or width % (4 * f):
             raise ValueError(f"height and width must be multiples of {4 * f} (feature maps are down-scaled {f}x, then twice more by 2)")
@@ -165,7 +128,7 @@ class ConvNet_TPS(_Module):
         S["gridGen.target_coordinate_repr"] = (self.height * self.width, n)
         return S
 
-    def _pack(self):
+    def _pack_weights(self):
         g, P = self._g, {}
         for name, cin in (("extractionA", 3), ("extractionB", self.input_nc)):
             layers = []
@@ -238,7 +201,6 @@ class ConvNet_TPS(_Module):
 
 class UNetVanilla(_Module):
     def __init__(self, n_channels, n_classes, bilinear=False, widths=(64, 128, 256, 512, 1024)):
-        super().__init__()
         if not bilinear:
             raise NotImplementedError("only the bilinear-upsampling variant built by the reference hub constructor (hubconf.py:58) exists")
         self.n_channels, self.n_classes, self.bilinear, self.widths = n_channels, n_classes, bilinear, tuple(widths)
@@ -261,7 +223,7 @@ class UNetVanilla(_Module):
         S["outc.conv.weight"], S["outc.conv.bias"] = (self.n_classes, self.widths[0], 1, 1), (self.n_classes,)
         return S
 
-    def _pack(self):
+    def _pack_weights(self):
         g, P = self._g, {}
         for p, srcs, mid, out in self._blocks():
             s1, t1 = self._bn(p + ".1")
