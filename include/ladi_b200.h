@@ -380,6 +380,27 @@ LADI_API int ladi_ssim_f32(const float* x, const float* y, int n, int c, int h, 
  * (source coordinate o * in/out, no half-pixel offset, upper neighbour clamped): x NCHW fp32 in [0, 1] -> out NCHW fp32 [n, c, oh, ow].
  * x and out 4-byte aligned (LADI_ERR_INVALID otherwise). */
 LADI_API int ladi_resize_tf1_u8(const float* x, int n, int c, int h, int w, int oh, int ow, float* out, void* stream);
+/* fp32 forms of the metric networks (metrics.py, precision="tf32": fp32 NHWC activations, every convolution a TF32 tensor-core GEMM
+ * with fp32 accumulation, as cuDNN runs the reference's fp32 convolutions by default on Ampere and Hopper).
+ * ladi_gemm_tf32: out[m, c_off + j] = relu?(sum_k a[m, k] w[j, k] + bias[j]) for j < n; a fp32 [m, a_pitch], w fp32 [n, w_pitch] (the
+ * K-major [c_out, K] convolution weight), bias fp32 [n] or NULL, relu 0 | 1, out fp32 of row pitch out_pitch (a block's NHWC
+ * concatenation; columns outside [c_off, c_off + n) untouched).  Both operands are rounded to TF32 to nearest (cvt.rna: 10 explicit
+ * mantissa bits, ties away from zero) inside the kernel, so each product is within 2^-10 relative of the fp32 operands' product;
+ * the sum is fp32 in K order (two runs give the same bits).  Columns k..a_pitch of `a` and k..w_pitch of `w` are never read (a K padded to a
+ * multiple of 4 with zeros is the packed layout).  Placement rules (LADI_ERR_INVALID, naming the operand): a and w 16-byte aligned with
+ * pitches >= k that are multiples of 4; n, c_off and out_pitch multiples of 4 with c_off + n <= out_pitch; out 16-byte aligned; bias 4-byte
+ * aligned; at most 65535 tiles of 128 rows (m <= 8388480).
+ * ladi_im2col_f32, ladi_pool2d_f32, ladi_lpips_layer_f32: ladi_im2col_bf16, ladi_pool2d_bf16 and ladi_lpips_layer on fp32 activations,
+ * with 4 in place of 8 in the channel, pitch, k_pad and c_off rules; the pixel form's out is fp32 (no rounding after the fp32 affine)
+ * and 4-byte aligned; lpips fa / fb 4-byte aligned.  GLOBAL_AVG_F32 reads fp32 x (4-byte aligned). */
+LADI_API int ladi_gemm_tf32(const float* a, int m, int k, int a_pitch, const float* w, int n, int w_pitch, const float* bias, int relu, float* out,
+                            int out_pitch, int c_off, void* stream);
+LADI_API int ladi_im2col_f32(const float* x, int x_is_nchw_pixels, int n, int c, int h, int w, int pitch, int kh, int kw, int sh, int sw, int ph,
+                             int pw, const float* shift, const float* scale, float* out, int k_pad, void* stream);
+LADI_API int ladi_pool2d_f32(const float* x, int n, int h, int w, int c, int x_pitch, int k, int s, int p, int mode, float* out, int out_pitch,
+                             int c_off, void* stream);
+LADI_API int ladi_lpips_layer_f32(const float* fa, const float* fb, int n, int h, int w, int c, int pitch, const float* lin, float* acc,
+                                  void* stream);
 
 /* ================================================================================================================================
  * Module-level ABI (SURVEY.md section 8(b)): an opaque per-device engine handle + one entry point per module of the try-on path.

@@ -39,8 +39,8 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-int ladi_encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                          const uint32_t* box, int swizzle_bytes) {
+static int encode_tmap(CUtensorMapDataType dtype, CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
+                       const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes) {
   EncodeTiledFn enc = get_encode();
   if (!enc) {
     ladi_set_error("cuTensorMapEncodeTiled unavailable (no CUDA driver?)");
@@ -64,7 +64,7 @@ int ladi_encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const ui
       }
     }
   }
-  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), d, s, b, e,
+  CUresult r = enc(out, dtype, (cuuint32_t)rank, const_cast<void*>(base), d, s, b, e,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -76,6 +76,16 @@ int ladi_encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const ui
     return LADI_ERR_CUDA;
   }
   return LADI_OK;
+}
+
+int ladi_encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                          const uint32_t* box, int swizzle_bytes) {
+  return encode_tmap(CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, out, base, rank, dims, strides_bytes, box, swizzle_bytes);
+}
+
+int ladi_encode_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                         const uint32_t* box) {
+  return encode_tmap(CU_TENSOR_MAP_DATA_TYPE_FLOAT32, out, base, rank, dims, strides_bytes, box, 128);
 }
 
 int ladi_num_sms() {

@@ -35,6 +35,9 @@ void ladi_set_error(const char* fmt, ...);
 // dims 1..rank-1.  Returns 0 on success.
 int ladi_encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                           const uint32_t* box, int swizzle_bytes = 128);
+// The same for fp32 elements (box[0] * 4 <= 128 bytes under the 128-byte swizzle).
+int ladi_encode_tmap_f32(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                         const uint32_t* box);
 
 int ladi_num_sms();
 void ladi_count_launch();  // every successful kernel launch of the library (ladi_launch / ladi_launch_cluster) -> ladi_launch_count()

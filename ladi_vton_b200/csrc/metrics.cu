@@ -1,7 +1,8 @@
 // Kernels of the image-quality metrics (ladi_vton_b200/metrics.py, the engine form of the reference's src/utils/val_metrics.py):
-// the im2col / pooling glue of the FID Inception-v3 and of the LPIPS AlexNet (their convolutions run on the wgmma GEMM, convgemm.cu),
-// the LPIPS distance layer, SSIM, and torch-fidelity's TF1-style bilinear resize for the Inception Score.  Every reduction has a fixed
-// order (no floating-point atomics), so two runs give identical bits.
+// the im2col / pooling glue of the FID Inception-v3 and of the LPIPS AlexNet (their convolutions run on the wgmma GEMMs: convgemm.cu for
+// bf16 activations, gemm_tf32.cu for fp32), the LPIPS distance layer, SSIM, and torch-fidelity's TF1-style bilinear resize for the
+// Inception Score.  The im2col, pooling and LPIPS kernels are templates on the activation type (bf16 or fp32); a thread moves 16 bytes
+// of channels (8 bf16 or 4 fp32).  Every reduction has a fixed order (no floating-point atomics), so two runs give identical bits.
 #include "common.h"
 #include "ptx.cuh"
 
@@ -13,15 +14,47 @@ inline int grid_for(long long total) {
   return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 
-// NHWC bf16 [n,h,w,pitch] -> rows [n*oh*ow, k_pad], column (ky*kw + kx)*c + ch, 8 channels (16 bytes) per thread; c % 8 == 0.
-__global__ void __launch_bounds__(256) im2col_nhwc_kernel(const bf16* __restrict__ x, int h, int w, int c, int pitch, int kh, int kw, int sh,
-                                                          int sw, int ph, int pw, int oh, int ow, long long rows, bf16* __restrict__ out,
+// 16 bytes of activations as floats: 8 bf16 or 4 fp32
+template <typename T> struct Vec16;
+template <> struct Vec16<bf16> {
+  static constexpr int N = 8, LOG_N = 3;
+  __device__ __forceinline__ static void unpack(uint4 u, float (&f)[8]) {
+    f[0] = ptx::bf16_lo(u.x); f[1] = ptx::bf16_hi(u.x); f[2] = ptx::bf16_lo(u.y); f[3] = ptx::bf16_hi(u.y);
+    f[4] = ptx::bf16_lo(u.z); f[5] = ptx::bf16_hi(u.z); f[6] = ptx::bf16_lo(u.w); f[7] = ptx::bf16_hi(u.w);
+  }
+  __device__ __forceinline__ static uint4 pack(const float (&f)[8]) {
+    uint4 r;
+    r.x = ptx::pack_bf16(f[0], f[1]); r.y = ptx::pack_bf16(f[2], f[3]);
+    r.z = ptx::pack_bf16(f[4], f[5]); r.w = ptx::pack_bf16(f[6], f[7]);
+    return r;
+  }
+};
+template <> struct Vec16<float> {
+  static constexpr int N = 4, LOG_N = 2;
+  __device__ __forceinline__ static void unpack(uint4 u, float (&f)[4]) {
+    f[0] = __uint_as_float(u.x); f[1] = __uint_as_float(u.y); f[2] = __uint_as_float(u.z); f[3] = __uint_as_float(u.w);
+  }
+  __device__ __forceinline__ static uint4 pack(const float (&f)[4]) {
+    return make_uint4(__float_as_uint(f[0]), __float_as_uint(f[1]), __float_as_uint(f[2]), __float_as_uint(f[3]));
+  }
+};
+__device__ __forceinline__ float to_f32(bf16 v) { return __bfloat162float(v); }
+__device__ __forceinline__ float to_f32(float v) { return v; }
+template <typename T> __device__ __forceinline__ T from_f32(float v);
+template <> __device__ __forceinline__ bf16 from_f32<bf16>(float v) { return __float2bfloat16(v); }
+template <> __device__ __forceinline__ float from_f32<float>(float v) { return v; }
+
+// NHWC [n,h,w,pitch] -> rows [n*oh*ow, k_pad], column (ky*kw + kx)*c + ch, 16 bytes of channels per thread; c % V == 0.
+template <typename T>
+__global__ void __launch_bounds__(256) im2col_nhwc_kernel(const T* __restrict__ x, int h, int w, int c, int pitch, int kh, int kw, int sh,
+                                                          int sw, int ph, int pw, int oh, int ow, long long rows, T* __restrict__ out,
                                                           int k_pad) {
   ptx::pdl_wait();
-  const int groups = k_pad >> 3, k_true = kh * kw * c;
+  constexpr int V = Vec16<T>::N;
+  const int groups = k_pad >> Vec16<T>::LOG_N, k_true = kh * kw * c;
   const long long total = rows * groups;
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
-    const int col = (int)(i % groups) * 8;
+    const int col = (int)(i % groups) * V;
     const long long r = i / groups;
     uint4 v = make_uint4(0u, 0u, 0u, 0u);
     if (col < k_true) {
@@ -37,9 +70,10 @@ __global__ void __launch_bounds__(256) im2col_nhwc_kernel(const bf16* __restrict
 }
 
 // NCHW fp32 pixels -> the same rows; (x - shift[ch]) / scale[ch] is applied to in-image pixels BEFORE the zero padding.
+template <typename T>
 __global__ void __launch_bounds__(256) im2col_pixels_kernel(const float* __restrict__ x, int c, int h, int w, int kh, int kw, int sh, int sw,
                                                             int ph, int pw, int oh, int ow, long long rows, const float* __restrict__ shift,
-                                                            const float* __restrict__ scale, bf16* __restrict__ out, int k_pad) {
+                                                            const float* __restrict__ scale, T* __restrict__ out, int k_pad) {
   ptx::pdl_wait();
   const int k_true = kh * kw * c;
   const long long total = rows * k_pad;
@@ -54,16 +88,18 @@ __global__ void __launch_bounds__(256) im2col_pixels_kernel(const float* __restr
       const int iy = oy * sh - ph + ky, ix = ox * sw - pw + kx;
       if (iy >= 0 && iy < h && ix >= 0 && ix < w) v = (__ldg(x + ((b * c + ch) * h + iy) * w + ix) - __ldg(shift + ch)) / __ldg(scale + ch);
     }
-    out[i] = __float2bfloat16(v);
+    out[i] = from_f32<T>(v);
   }
 }
 
-// torch max_pool2d / avg_pool2d (ceil_mode=False) on NHWC bf16, 8 channels per thread, output into channels [c_off, c_off + c) of
+// torch max_pool2d / avg_pool2d (ceil_mode=False) on NHWC, 16 bytes of channels per thread, output into channels [c_off, c_off + c) of
 // `out` [n, oh, ow, out_pitch].  Average: fp32 sum in window order, divided by the window size counted as torch does.
-__global__ void __launch_bounds__(256) pool2d_kernel(const bf16* __restrict__ x, int h, int w, int c, int pitch, int k, int s, int p, int mode,
-                                                     int oh, int ow, long long pixels, bf16* __restrict__ out, int out_pitch, int c_off) {
+template <typename T>
+__global__ void __launch_bounds__(256) pool2d_kernel(const T* __restrict__ x, int h, int w, int c, int pitch, int k, int s, int p, int mode,
+                                                     int oh, int ow, long long pixels, T* __restrict__ out, int out_pitch, int c_off) {
   ptx::pdl_wait();
-  const int nv = c >> 3;
+  constexpr int V = Vec16<T>::N;
+  const int nv = c >> Vec16<T>::LOG_N;
   const long long total = pixels * nv;
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
     const int v = (int)(i % nv);
@@ -74,40 +110,37 @@ __global__ void __launch_bounds__(256) pool2d_kernel(const bf16* __restrict__ x,
     int y1 = min(y0 + k, h + p), x1 = min(x0 + k, w + p);
     const int padded = (y1 - y0) * (x1 - x0);
     y0 = max(y0, 0); x0 = max(x0, 0); y1 = min(y1, h); x1 = min(x1, w);
-    float acc[8];
+    float acc[V];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) acc[j] = mode == LADI_POOL_MAX ? -INFINITY : 0.f;
+    for (int j = 0; j < V; ++j) acc[j] = mode == LADI_POOL_MAX ? -INFINITY : 0.f;
     for (int yy = y0; yy < y1; ++yy)
       for (int xx = x0; xx < x1; ++xx) {
-        const uint4 u = __ldg(reinterpret_cast<const uint4*>(x + ((b * h + yy) * w + xx) * pitch + v * 8));
-        const float f[8] = {ptx::bf16_lo(u.x), ptx::bf16_hi(u.x), ptx::bf16_lo(u.y), ptx::bf16_hi(u.y),
-                            ptx::bf16_lo(u.z), ptx::bf16_hi(u.z), ptx::bf16_lo(u.w), ptx::bf16_hi(u.w)};
+        float f[V];
+        Vec16<T>::unpack(__ldg(reinterpret_cast<const uint4*>(x + ((b * h + yy) * w + xx) * pitch + v * V)), f);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) acc[j] = mode == LADI_POOL_MAX ? fmaxf(acc[j], f[j]) : acc[j] + f[j];
+        for (int j = 0; j < V; ++j) acc[j] = mode == LADI_POOL_MAX ? fmaxf(acc[j], f[j]) : acc[j] + f[j];
       }
     if (mode != LADI_POOL_MAX) {
       const float inv = 1.f / (float)(mode == LADI_POOL_AVG ? padded : (y1 - y0) * (x1 - x0));
 #pragma unroll
-      for (int j = 0; j < 8; ++j) acc[j] *= inv;
+      for (int j = 0; j < V; ++j) acc[j] *= inv;
     }
-    uint4 r;
-    r.x = ptx::pack_bf16(acc[0], acc[1]); r.y = ptx::pack_bf16(acc[2], acc[3]);
-    r.z = ptx::pack_bf16(acc[4], acc[5]); r.w = ptx::pack_bf16(acc[6], acc[7]);
-    *reinterpret_cast<uint4*>(out + px * out_pitch + c_off + v * 8) = r;
+    *reinterpret_cast<uint4*>(out + px * out_pitch + c_off + v * V) = Vec16<T>::pack(acc);
   }
 }
 
 // adaptive_avg_pool2d(x, 1).flatten(1): out fp32 [n, out_pitch], one thread per (image, channel), pixels summed in order.
-__global__ void __launch_bounds__(256) global_avg_kernel(const bf16* __restrict__ x, int n, int hw, int c, int pitch, float* __restrict__ out,
+template <typename T>
+__global__ void __launch_bounds__(256) global_avg_kernel(const T* __restrict__ x, int n, int hw, int c, int pitch, float* __restrict__ out,
                                                          int out_pitch) {
   ptx::pdl_wait();
   const long long total = (long long)n * c;
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
     const int ch = (int)(i % c);
     const long long b = i / c;
-    const bf16* p = x + b * hw * pitch + ch;
+    const T* p = x + b * hw * pitch + ch;
     float acc = 0.f;
-    for (int q = 0; q < hw; ++q) acc += __bfloat162float(p[(long long)q * pitch]);
+    for (int q = 0; q < hw; ++q) acc += to_f32(p[(long long)q * pitch]);
     out[b * out_pitch + ch] = acc / (float)hw;
   }
 }
@@ -115,20 +148,21 @@ __global__ void __launch_bounds__(256) global_avg_kernel(const bf16* __restrict_
 // One LPIPS layer (lpips.LPIPS.forward, version 0.1): per pixel na = a / (|a| + 1e-10), nb likewise, d = sum_c lin[c] (na - nb)^2;
 // acc[b] += mean over pixels of d.  One block per image; warp w takes pixels w, w + 16, ...; warps combined in index order.
 constexpr int LPIPS_WARPS = 16;
-__global__ void __launch_bounds__(LPIPS_WARPS * 32) lpips_layer_kernel(const bf16* __restrict__ fa, const bf16* __restrict__ fb, int hw, int c,
+template <typename T>
+__global__ void __launch_bounds__(LPIPS_WARPS * 32) lpips_layer_kernel(const T* __restrict__ fa, const T* __restrict__ fb, int hw, int c,
                                                                        int pitch, const float* __restrict__ lin, float* __restrict__ acc) {
   ptx::pdl_wait();
   __shared__ float part[LPIPS_WARPS];
   const int b = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const bf16* A = fa + (long long)b * hw * pitch;
-  const bf16* B = fb + (long long)b * hw * pitch;
+  const T* A = fa + (long long)b * hw * pitch;
+  const T* B = fb + (long long)b * hw * pitch;
   float mine = 0.f;
   for (int q = warp; q < hw; q += LPIPS_WARPS) {
-    const bf16* pa = A + (long long)q * pitch;
-    const bf16* pb = B + (long long)q * pitch;
+    const T* pa = A + (long long)q * pitch;
+    const T* pb = B + (long long)q * pitch;
     float sa = 0.f, sb = 0.f;
     for (int ch = lane; ch < c; ch += 32) {
-      const float a = __bfloat162float(pa[ch]), bb = __bfloat162float(pb[ch]);
+      const float a = to_f32(pa[ch]), bb = to_f32(pb[ch]);
       sa = fmaf(a, a, sa);
       sb = fmaf(bb, bb, sb);
     }
@@ -140,7 +174,7 @@ __global__ void __launch_bounds__(LPIPS_WARPS * 32) lpips_layer_kernel(const bf1
     const float ra = 1.f / (sqrtf(sa) + 1e-10f), rb = 1.f / (sqrtf(sb) + 1e-10f);
     float d = 0.f;
     for (int ch = lane; ch < c; ch += 32) {
-      const float t = __bfloat162float(pa[ch]) * ra - __bfloat162float(pb[ch]) * rb;
+      const float t = to_f32(pa[ch]) * ra - to_f32(pb[ch]) * rb;
       d = fmaf(__ldg(lin + ch), t * t, d);
     }
 #pragma unroll
@@ -282,14 +316,14 @@ extern "C" int ladi_im2col_bf16(const void* x, int x_is_f32_nchw, int n, int c, 
     LADI_CHECK(aligned_to(shift, 4), "im2col: shift %p must be 4-byte aligned", shift);
     LADI_CHECK(aligned_to(scale, 4), "im2col: scale %p must be 4-byte aligned", scale);
     LADI_CHECK(aligned_to(out, 2), "im2col: out %p must be 2-byte aligned", out);
-    LADI_CUDA(ladi_launch(im2col_pixels_kernel, dim3(grid_for(rows * k_pad)), dim3(256), 0, STREAM, (const float*)x, c, h, w, kh, kw, sh, sw, ph,
+    LADI_CUDA(ladi_launch(im2col_pixels_kernel<bf16>, dim3(grid_for(rows * k_pad)), dim3(256), 0, STREAM, (const float*)x, c, h, w, kh, kw, sh, sw, ph,
                           pw, oh, ow, rows, shift, scale, (bf16*)out, k_pad));
   } else {
     LADI_CHECK(!shift && !scale, "im2col: shift / scale apply to the fp32 pixel form only");
     LADI_CHECK(c % 8 == 0 && pitch % 8 == 0 && pitch >= c, "im2col: C and pitch must be multiples of 8");
     LADI_CHECK(aligned_to(x, 16), "im2col: x %p must be 16-byte aligned", x);
     LADI_CHECK(aligned_to(out, 16), "im2col: out %p must be 16-byte aligned", out);
-    LADI_CUDA(ladi_launch(im2col_nhwc_kernel, dim3(grid_for(rows * (k_pad / 8))), dim3(256), 0, STREAM, (const bf16*)x, h, w, c, pitch, kh, kw, sh,
+    LADI_CUDA(ladi_launch(im2col_nhwc_kernel<bf16>, dim3(grid_for(rows * (k_pad / 8))), dim3(256), 0, STREAM, (const bf16*)x, h, w, c, pitch, kh, kw, sh,
                           sw, ph, pw, oh, ow, rows, (bf16*)out, k_pad));
   }
   return LADI_OK;
@@ -303,7 +337,7 @@ extern "C" int ladi_pool2d_bf16(const void* x, int n, int h, int w, int c, int x
     LADI_CHECK(out_pitch >= c_off + c, "pool2d: channel window outside the output pitch");
     LADI_CHECK(aligned_to(x, 2), "pool2d: x %p must be 2-byte aligned", x);
     LADI_CHECK(aligned_to(out, 4), "pool2d: out %p must be 4-byte aligned (fp32 features)", out);
-    LADI_CUDA(ladi_launch(global_avg_kernel, dim3(grid_for((long long)n * c)), dim3(256), 0, STREAM, (const bf16*)x, n, h * w, c, x_pitch,
+    LADI_CUDA(ladi_launch(global_avg_kernel<bf16>, dim3(grid_for((long long)n * c)), dim3(256), 0, STREAM, (const bf16*)x, n, h * w, c, x_pitch,
                           (float*)out + c_off, out_pitch));
     return LADI_OK;
   }
@@ -314,7 +348,7 @@ extern "C" int ladi_pool2d_bf16(const void* x, int n, int h, int w, int c, int x
   LADI_CHECK(aligned_to(out, 16), "pool2d: out %p must be 16-byte aligned", out);
   const int oh = (h + 2 * p - k) / s + 1, ow = (w + 2 * p - k) / s + 1;
   const long long pixels = (long long)n * oh * ow;
-  LADI_CUDA(ladi_launch(pool2d_kernel, dim3(grid_for(pixels * (c / 8))), dim3(256), 0, STREAM, (const bf16*)x, h, w, c, x_pitch, k, s, p, mode, oh,
+  LADI_CUDA(ladi_launch(pool2d_kernel<bf16>, dim3(grid_for(pixels * (c / 8))), dim3(256), 0, STREAM, (const bf16*)x, h, w, c, x_pitch, k, s, p, mode, oh,
                         ow, pixels, (bf16*)out, out_pitch, c_off));
   return LADI_OK;
 }
@@ -325,7 +359,69 @@ extern "C" int ladi_lpips_layer(const void* fa, const void* fb, int n, int h, in
   LADI_CHECK(aligned_to(fb, 2), "lpips_layer: fb %p must be 2-byte aligned", fb);
   LADI_CHECK(aligned_to(lin, 4), "lpips_layer: lin %p must be 4-byte aligned", lin);
   LADI_CHECK(aligned_to(acc, 4), "lpips_layer: acc %p must be 4-byte aligned", acc);
-  LADI_CUDA(ladi_launch(lpips_layer_kernel, dim3(n), dim3(LPIPS_WARPS * 32), 0, STREAM, (const bf16*)fa, (const bf16*)fb, h * w, c, pitch, lin, acc));
+  LADI_CUDA(ladi_launch(lpips_layer_kernel<bf16>, dim3(n), dim3(LPIPS_WARPS * 32), 0, STREAM, (const bf16*)fa, (const bf16*)fb, h * w, c, pitch, lin, acc));
+  return LADI_OK;
+}
+
+extern "C" int ladi_im2col_f32(const float* x, int x_is_nchw_pixels, int n, int c, int h, int w, int pitch, int kh, int kw, int sh, int sw,
+                               int ph, int pw, const float* shift, const float* scale, float* out, int k_pad, void* stream) {
+  LADI_CHECK(x && out && n > 0 && c > 0 && h > 0 && w > 0 && kh > 0 && kw > 0 && sh > 0 && sw > 0 && ph >= 0 && pw >= 0,
+             "im2col_f32: bad extent");
+  const int oh = (h + 2 * ph - kh) / sh + 1, ow = (w + 2 * pw - kw) / sw + 1;
+  LADI_CHECK(h + 2 * ph >= kh && w + 2 * pw >= kw && oh > 0 && ow > 0, "im2col_f32: window larger than the padded image");
+  LADI_CHECK(k_pad % 4 == 0 && k_pad >= kh * kw * c, "im2col_f32: k_pad must be a multiple of 4 and >= kh*kw*c");
+  const long long rows = (long long)n * oh * ow;
+  if (x_is_nchw_pixels) {
+    LADI_CHECK(shift && scale, "im2col_f32: the pixel form needs shift and scale");
+    LADI_CHECK(aligned_to(x, 4), "im2col_f32: x %p must be 4-byte aligned", x);
+    LADI_CHECK(aligned_to(shift, 4), "im2col_f32: shift %p must be 4-byte aligned", shift);
+    LADI_CHECK(aligned_to(scale, 4), "im2col_f32: scale %p must be 4-byte aligned", scale);
+    LADI_CHECK(aligned_to(out, 4), "im2col_f32: out %p must be 4-byte aligned", out);
+    LADI_CUDA(ladi_launch(im2col_pixels_kernel<float>, dim3(grid_for(rows * k_pad)), dim3(256), 0, STREAM, x, c, h, w, kh, kw, sh, sw, ph, pw,
+                          oh, ow, rows, shift, scale, out, k_pad));
+  } else {
+    LADI_CHECK(!shift && !scale, "im2col_f32: shift / scale apply to the pixel form only");
+    LADI_CHECK(c % 4 == 0 && pitch % 4 == 0 && pitch >= c, "im2col_f32: C and pitch must be multiples of 4");
+    LADI_CHECK(aligned_to(x, 16), "im2col_f32: x %p must be 16-byte aligned", x);
+    LADI_CHECK(aligned_to(out, 16), "im2col_f32: out %p must be 16-byte aligned", out);
+    LADI_CUDA(ladi_launch(im2col_nhwc_kernel<float>, dim3(grid_for(rows * (k_pad / 4))), dim3(256), 0, STREAM, x, h, w, c, pitch, kh, kw, sh, sw,
+                          ph, pw, oh, ow, rows, out, k_pad));
+  }
+  return LADI_OK;
+}
+
+extern "C" int ladi_pool2d_f32(const float* x, int n, int h, int w, int c, int x_pitch, int k, int s, int p, int mode, float* out, int out_pitch,
+                               int c_off, void* stream) {
+  LADI_CHECK(x && out && n > 0 && h > 0 && w > 0 && c > 0, "pool2d_f32: bad extent");
+  LADI_CHECK(c % 4 == 0 && x_pitch % 4 == 0 && x_pitch >= c, "pool2d_f32: C and pitch must be multiples of 4");
+  if (mode == LADI_POOL_GLOBAL_AVG_F32) {
+    LADI_CHECK(out_pitch >= c_off + c, "pool2d_f32: channel window outside the output pitch");
+    LADI_CHECK(aligned_to(x, 4), "pool2d_f32: x %p must be 4-byte aligned", x);
+    LADI_CHECK(aligned_to(out, 4), "pool2d_f32: out %p must be 4-byte aligned", out);
+    LADI_CUDA(ladi_launch(global_avg_kernel<float>, dim3(grid_for((long long)n * c)), dim3(256), 0, STREAM, x, n, h * w, c, x_pitch, out + c_off,
+                          out_pitch));
+    return LADI_OK;
+  }
+  LADI_CHECK(mode == LADI_POOL_MAX || mode == LADI_POOL_AVG || mode == LADI_POOL_AVG_EXCLUDE_PAD, "pool2d_f32: unknown mode %d", mode);
+  LADI_CHECK(k > 0 && s > 0 && p >= 0 && 2 * p <= k && h + 2 * p >= k && w + 2 * p >= k, "pool2d_f32: bad window (k %d, s %d, p %d)", k, s, p);
+  LADI_CHECK(out_pitch % 4 == 0 && c_off % 4 == 0 && out_pitch >= c_off + c, "pool2d_f32: output pitch / channel offset must be multiples of 4");
+  LADI_CHECK(aligned_to(x, 16), "pool2d_f32: x %p must be 16-byte aligned", x);
+  LADI_CHECK(aligned_to(out, 16), "pool2d_f32: out %p must be 16-byte aligned", out);
+  const int oh = (h + 2 * p - k) / s + 1, ow = (w + 2 * p - k) / s + 1;
+  const long long pixels = (long long)n * oh * ow;
+  LADI_CUDA(ladi_launch(pool2d_kernel<float>, dim3(grid_for(pixels * (c / 4))), dim3(256), 0, STREAM, x, h, w, c, x_pitch, k, s, p, mode, oh, ow,
+                        pixels, out, out_pitch, c_off));
+  return LADI_OK;
+}
+
+extern "C" int ladi_lpips_layer_f32(const float* fa, const float* fb, int n, int h, int w, int c, int pitch, const float* lin, float* acc,
+                                    void* stream) {
+  LADI_CHECK(fa && fb && lin && acc && n > 0 && h > 0 && w > 0 && c > 0 && pitch >= c, "lpips_layer_f32: bad extent");
+  LADI_CHECK(aligned_to(fa, 4), "lpips_layer_f32: fa %p must be 4-byte aligned", fa);
+  LADI_CHECK(aligned_to(fb, 4), "lpips_layer_f32: fb %p must be 4-byte aligned", fb);
+  LADI_CHECK(aligned_to(lin, 4), "lpips_layer_f32: lin %p must be 4-byte aligned", lin);
+  LADI_CHECK(aligned_to(acc, 4), "lpips_layer_f32: acc %p must be 4-byte aligned", acc);
+  LADI_CUDA(ladi_launch(lpips_layer_kernel<float>, dim3(n), dim3(LPIPS_WARPS * 32), 0, STREAM, fa, fb, h * w, c, pitch, lin, acc));
   return LADI_OK;
 }
 

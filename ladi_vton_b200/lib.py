@@ -132,6 +132,10 @@ SIGNATURES = {
     "ladi_ssim_partials": ([_I, _I], _I),
     "ladi_ssim_f32": ([_P, _P, _I, _I, _I, _I, _P, _P, _P], _I),
     "ladi_resize_tf1_u8": ([_P, _I, _I, _I, _I, _I, _I, _P, _P], _I),
+    "ladi_gemm_tf32": ([_P, _I, _I, _I, _P, _I, _I, _P, _I, _P, _I, _I, _P], _I),
+    "ladi_im2col_f32": ([_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _I, _P], _I),
+    "ladi_pool2d_f32": ([_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _I, _I, _P], _I),
+    "ladi_lpips_layer_f32": ([_P, _P, _I, _I, _I, _I, _I, _P, _P, _P], _I),
     # ---- module-level ABI (csrc/engine.cu)
     "ladi_engine_create": ([C.POINTER(EngineConfig), C.POINTER(Weight), _I, _PP], _I),
     "ladi_engine_destroy": ([_P], _I),

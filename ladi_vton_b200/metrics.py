@@ -18,6 +18,12 @@ strided 3x3, and 3x3 at odd widths, where the implicit path's 128-row tile would
 Branch outputs and pools are written straight into their block's channel concatenation.  Activations are bf16 with fp32 accumulation; the
 input affine ((x - 128) / 128 for Inception, the LPIPS scaling layer for AlexNet) is applied in fp32 by the pixel im2col before the
 padding.  No CPU path: `.to("cpu")` raises.
+
+`precision="tf32"` (both networks' constructors; the default is "bf16") is the precision the reference computes in on a GPU: clean-fid's and
+torchmetrics' fp32 modules under PyTorch's default `torch.backends.cudnn.allow_tf32 = True`.  Activations are fp32 NHWC, the weights fp32
+(BatchNorm folded in float64, K padded with zeros to a multiple of 4), and every convolution is one `ladi_gemm_tf32` (TF32 tensor cores,
+operands rounded to nearest TF32 inside the kernel, fp32 accumulation): a 1x1 convolution directly over the NHWC rows, every other one
+over `ladi_im2col_f32` rows.  Pools and the LPIPS layers run their fp32 forms.
 """
 import math
 
@@ -28,6 +34,7 @@ from . import lib, ops
 from .module import PackedModule
 from .weights import pad64
 
+PRECISIONS = ("bf16", "tf32")
 INCEPTION_BN_EPS = 1e-3
 INCEPTION_FILE = "pt_inception-2015-12-05-6726825d.pth"
 ALEXNET_FILE = "alexnet-owt-7be5be79.pth"
@@ -35,6 +42,10 @@ LPIPS_FILE = "alex.pth"
 # LPIPS ScalingLayer (lpips/pretrained_networks.py, v0.1): (x - shift) / scale on [-1, 1] images
 LPIPS_SHIFT = (-0.030, -0.088, -0.188)
 LPIPS_SCALE = (0.458, 0.448, 0.450)
+
+
+def pad4(k):
+    return (k + 3) // 4 * 4
 
 
 def _pair(v):
@@ -109,13 +120,14 @@ def uses_implicit_3x3(kernel, stride, padding, w_out):
     return kernel == (3, 3) and stride == (1, 1) and padding == (1, 1) and w_out % 8 == 0
 
 
-def pack_im2col_weight(w):
-    """[c_out, c_in, kh, kw] -> bf16 [c_out, pad64(kh*kw*c_in)] in ladi_im2col_bf16's (ky, kx, c) column order."""
+def pack_im2col_weight(w, dtype=torch.bfloat16):
+    """[c_out, c_in, kh, kw] -> [c_out, K'] in the im2col (ky, kx, c) column order, zeros in the columns past kh*kw*c_in: bf16 with
+    K' = pad64(kh*kw*c_in) for ladi_conv2d_bf16, or fp32 with K' = pad4(kh*kw*c_in) for ladi_gemm_tf32."""
     co, ci, kh, kw = w.shape
     flat = w.permute(0, 2, 3, 1).reshape(co, kh * kw * ci)
-    out = flat.new_zeros((co, pad64(kh * kw * ci)))
+    out = flat.new_zeros((co, (pad4 if dtype == torch.float32 else pad64)(kh * kw * ci)))
     out[:, :flat.shape[1]] = flat
-    return out.to(torch.bfloat16).contiguous()
+    return out.to(dtype).contiguous()
 
 
 def fold_bn(w, gamma, beta, mean, var, eps):
@@ -125,21 +137,28 @@ def fold_bn(w, gamma, beta, mean, var, eps):
 
 
 class _Conv:
-    """One convolution + ReLU, packed for both paths (the choice needs the output width, known at call time)."""
+    """One convolution + ReLU.  bf16: packed for both paths (the choice needs the output width, known at call time).  tf32: one fp32
+    [c_out, pad4(K)] weight for ladi_gemm_tf32, from the float64 `w`."""
 
-    def __init__(self, w, b, stride, padding, device):
+    def __init__(self, w, b, stride, padding, device, precision="bf16"):
         self.c_in, self.c_out = int(w.shape[1]), int(w.shape[0])
         self.kernel, self.stride, self.padding = tuple(w.shape[2:]), stride, padding
-        self.w_cols = pack_im2col_weight(w.float()).to(device)
+        self.tf32 = precision == "tf32"
+        self.bias = b.float().contiguous().to(device)
         self.w_3x3 = None
+        if self.tf32:
+            self.w_cols = pack_im2col_weight(w.double(), torch.float32).to(device)
+            return
+        self.w_cols = pack_im2col_weight(w.float()).to(device)
         if self.kernel == (3, 3) and stride == (1, 1) and padding == (1, 1):
             from .weights import pack_conv
             self.w_3x3 = pack_conv(w.float(), [self.c_in]).to(device)
-        self.bias = b.float().contiguous().to(device)
 
     def __call__(self, x, out=None, c_off=0, shift=None, scale=None):
-        """x NHWC bf16 [n, h, w, c_in] (or NCHW fp32 pixels with shift / scale) -> ReLU(conv) NHWC bf16, written to channels
-        [c_off, c_off + c_out) of `out` when given."""
+        """x NHWC bf16 [n, h, w, c_in] (fp32 with tf32; or NCHW fp32 pixels with shift / scale) -> ReLU(conv) NHWC bf16 (fp32 with tf32),
+        written to channels [c_off, c_off + c_out) of `out` when given."""
+        if self.tf32:
+            return self._call_tf32(x, out, c_off, shift, scale)
         if x.dtype == torch.float32:
             n, _, h, w = x.shape
         else:
@@ -160,9 +179,30 @@ class _Conv:
         ops.gemm(a, self.w_cols, self.c_out, bias=self.bias, act=ops.ACT_RELU, out=out.view(n * oh * ow, out.shape[3])[:, c_off:c_off + self.c_out])
         return out
 
+    def _call_tf32(self, x, out, c_off, shift, scale):
+        pixels = shift is not None
+        n, h, w = (x.shape[0], x.shape[2], x.shape[3]) if pixels else x.shape[:3]
+        oh = ops.conv_out_size(h, self.kernel[0], self.stride[0], self.padding[0])
+        ow = ops.conv_out_size(w, self.kernel[1], self.stride[1], self.padding[1])
+        if out is None:
+            out = torch.empty((n, oh, ow, self.c_out), dtype=torch.float32, device=x.device)
+        if self.kernel == (1, 1) and self.stride == (1, 1) and self.padding == (0, 0) and not pixels:
+            assert x.dtype == torch.float32 and x.is_contiguous()
+            a = x.view(n * h * w, self.c_in)
+        else:
+            a, _ = ops.im2col(x, self.kernel, self.stride, self.padding, self.w_cols.shape[1], shift=shift, scale=scale, dtype=torch.float32)
+        ops.gemm_tf32(a, self.w_cols, self.c_out, out.view(n * oh * ow, out.shape[3]), c_off, bias=self.bias, relu=True)
+        return out
+
 
 class _Net(PackedModule):
     layers = None
+
+    def __init__(self, precision="bf16"):
+        if precision not in PRECISIONS:
+            raise ValueError(f"{type(self).__name__}: precision must be one of {PRECISIONS}, got {precision!r}")
+        self.precision = precision
+        self.dtype = torch.float32 if precision == "tf32" else torch.bfloat16  # the activations'
 
     def _check_ready(self):
         if self.layers is None:
@@ -186,7 +226,7 @@ class FIDInceptionV3(_Net):
         for name, (_, _, _, s, p) in INCEPTION_LAYERS.items():
             w, b = fold_bn(sd[f"{name}.conv.weight"], sd[f"{name}.bn.weight"], sd[f"{name}.bn.bias"], sd[f"{name}.bn.running_mean"],
                            sd[f"{name}.bn.running_var"], INCEPTION_BN_EPS)
-            self.layers[name] = _Conv(w, b, s, p, dev)
+            self.layers[name] = _Conv(w, b, s, p, dev, self.precision)
         self.fc_weight = sd["fc.weight"].double().cpu()
         self.shift = torch.full((3,), 128.0, device=dev)
         self.scale = torch.full((3,), 128.0, device=dev)
@@ -195,7 +235,7 @@ class FIDInceptionV3(_Net):
         L = self.layers
         n, h, w, _ = x.shape
         pf = L[f"{m}.branch_pool"].c_out
-        out = torch.empty((n, h, w, 224 + pf), dtype=torch.bfloat16, device=x.device)
+        out = torch.empty((n, h, w, 224 + pf), dtype=self.dtype, device=x.device)
         L[f"{m}.branch1x1"](x, out, 0)
         L[f"{m}.branch5x5_2"](L[f"{m}.branch5x5_1"](x), out, 64)
         L[f"{m}.branch3x3dbl_3"](L[f"{m}.branch3x3dbl_2"](L[f"{m}.branch3x3dbl_1"](x)), out, 128)
@@ -206,7 +246,7 @@ class FIDInceptionV3(_Net):
         L = self.layers
         n, h, w, c = x.shape
         oh, ow = ops.conv_out_size(h, 3, 2, 0), ops.conv_out_size(w, 3, 2, 0)
-        out = torch.empty((n, oh, ow, 480 + c), dtype=torch.bfloat16, device=x.device)
+        out = torch.empty((n, oh, ow, 480 + c), dtype=self.dtype, device=x.device)
         L[f"{m}.branch3x3"](x, out, 0)
         L[f"{m}.branch3x3dbl_3"](L[f"{m}.branch3x3dbl_2"](L[f"{m}.branch3x3dbl_1"](x)), out, 384)
         ops.pool2d(x, 3, 2, 0, ops.POOL_MAX, out=out, c_off=480)
@@ -215,7 +255,7 @@ class FIDInceptionV3(_Net):
     def _block_c(self, x, m):
         L = self.layers
         n, h, w, _ = x.shape
-        out = torch.empty((n, h, w, 768), dtype=torch.bfloat16, device=x.device)
+        out = torch.empty((n, h, w, 768), dtype=self.dtype, device=x.device)
         L[f"{m}.branch1x1"](x, out, 0)
         L[f"{m}.branch7x7_3"](L[f"{m}.branch7x7_2"](L[f"{m}.branch7x7_1"](x)), out, 192)
         t = x
@@ -229,7 +269,7 @@ class FIDInceptionV3(_Net):
         L = self.layers
         n, h, w, c = x.shape
         oh, ow = ops.conv_out_size(h, 3, 2, 0), ops.conv_out_size(w, 3, 2, 0)
-        out = torch.empty((n, oh, ow, 512 + c), dtype=torch.bfloat16, device=x.device)
+        out = torch.empty((n, oh, ow, 512 + c), dtype=self.dtype, device=x.device)
         L[f"{m}.branch3x3_2"](L[f"{m}.branch3x3_1"](x), out, 0)
         t = x
         for i in range(1, 4):
@@ -241,7 +281,7 @@ class FIDInceptionV3(_Net):
     def _block_e(self, x, m, pool_mode):
         L = self.layers
         n, h, w, _ = x.shape
-        out = torch.empty((n, h, w, 2048), dtype=torch.bfloat16, device=x.device)
+        out = torch.empty((n, h, w, 2048), dtype=self.dtype, device=x.device)
         L[f"{m}.branch1x1"](x, out, 0)
         t = L[f"{m}.branch3x3_1"](x)
         L[f"{m}.branch3x3_2a"](t, out, 320)
@@ -299,7 +339,7 @@ class LPIPSAlex(_Net):
 
     def _pack_weights(self):
         sd, dev = self._sd, self.device
-        self.layers = {i: _Conv(sd[f"features.{i}.weight"].double(), sd[f"features.{i}.bias"].double(), s, p, dev)
+        self.layers = {i: _Conv(sd[f"features.{i}.weight"].double(), sd[f"features.{i}.bias"].double(), s, p, dev, self.precision)
                        for i, (_, _, _, s, p) in ALEX_LAYERS.items()}
         self.lins = [sd[f"lin{t}.model.1.weight"].reshape(-1).float().contiguous().to(dev) for t in range(5)]
         # [0,1] -> 2x - 1 -> (v - shift) / scale  ==  (x - (1 + shift) / 2) / (scale / 2)
@@ -308,7 +348,7 @@ class LPIPSAlex(_Net):
 
     @torch.no_grad()
     def taps(self, images01):
-        """AlexNet relu1..relu5 of NCHW fp32 images in [0, 1] (after the scaling layer): list of NHWC bf16 tensors."""
+        """AlexNet relu1..relu5 of NCHW fp32 images in [0, 1] (after the scaling layer): list of NHWC bf16 (fp32 with tf32) tensors."""
         self._check_ready()
         L = self.layers
         t1 = L[0](images01.contiguous(), shift=self.shift, scale=self.scale)

@@ -565,52 +565,70 @@ def conv_out_size(size, k, s, p):
     return (size + 2 * p - k) // s + 1
 
 
-def im2col(x, kernel, stride, padding, k_pad, shift=None, scale=None):
-    """Rows [n*oh*ow, k_pad] bf16, column (ky*kw + kx)*c + ch, of a kernel=(kh, kw) / stride=(sh, sw) / padding=(ph, pw) convolution.
-    x: NHWC bf16 (channel-sliced views fine, c % 8 == 0), or NCHW fp32 pixels with per-channel fp32 `shift` / `scale` applied as
-    (x - shift) / scale before the zero padding."""
+def im2col(x, kernel, stride, padding, k_pad, shift=None, scale=None, dtype=torch.bfloat16):
+    """Rows [n*oh*ow, k_pad] of `dtype` (bf16, or fp32 for the tf32 metric networks), column (ky*kw + kx)*c + ch, of a kernel=(kh, kw) /
+    stride=(sh, sw) / padding=(ph, pw) convolution.  x: NHWC of the same dtype (channel-sliced views fine, c % 8 == 0), or NCHW fp32
+    pixels (with shift / scale given) whose per-channel fp32 affine (x - shift) / scale is applied before the zero padding."""
     (kh, kw), (sh, sw), (ph, pw) = kernel, stride, padding
-    pixels = x.dtype == torch.float32
+    pixels = shift is not None
     if pixels:
-        assert x.is_contiguous() and shift is not None and scale is not None
+        assert x.dtype == torch.float32 and x.is_contiguous() and scale is not None
         n, c, h, w = x.shape
         pitch = 0
     else:
-        assert x.dtype == torch.bfloat16 and shift is None and scale is None
+        assert x.dtype == dtype and scale is None
         n, h, w, c, pitch = _nhwc(x)
     oh, ow = conv_out_size(h, kh, sh, ph), conv_out_size(w, kw, sw, pw)
-    out = torch.empty((n * oh * ow, k_pad), dtype=torch.bfloat16, device=x.device)
-    _call("ladi_im2col_bf16", 0.0, _ptr(x), int(pixels), n, c, h, w, pitch, kh, kw, sh, sw, ph, pw, _ptr(shift), _ptr(scale), _ptr(out), k_pad,
-          _stream())
+    out = torch.empty((n * oh * ow, k_pad), dtype=dtype, device=x.device)
+    name = "ladi_im2col_f32" if dtype == torch.float32 else "ladi_im2col_bf16"
+    _call(name, 0.0, _ptr(x), int(pixels), n, c, h, w, pitch, kh, kw, sh, sw, ph, pw, _ptr(shift), _ptr(scale), _ptr(out), k_pad, _stream())
     return out, (n, oh, ow)
 
 
+_POOL = {torch.bfloat16: "ladi_pool2d_bf16", torch.float32: "ladi_pool2d_f32"}
+_LPIPS = {torch.bfloat16: "ladi_lpips_layer", torch.float32: "ladi_lpips_layer_f32"}
+
+
 def pool2d(x, k, s, p, mode, out=None, c_off=0):
-    """torch max_pool2d / avg_pool2d on NHWC bf16; the result goes to channels [c_off, c_off + C) of `out` when given."""
+    """torch max_pool2d / avg_pool2d on NHWC bf16 or fp32; the result (same dtype) goes to channels [c_off, c_off + C) of `out` when
+    given."""
     n, h, w, c, pitch = _nhwc(x)
     oh, ow = conv_out_size(h, k, s, p), conv_out_size(w, k, s, p)
     if out is None:
-        out = torch.empty((n, oh, ow, c), dtype=torch.bfloat16, device=x.device)
-    assert out.dtype == torch.bfloat16 and out.is_contiguous() and tuple(out.shape[:3]) == (n, oh, ow) and out.shape[3] >= c_off + c
-    _call("ladi_pool2d_bf16", 0.0, _ptr(x), n, h, w, c, pitch, k, s, p, mode, _ptr(out), out.shape[3], c_off, _stream())
+        out = torch.empty((n, oh, ow, c), dtype=x.dtype, device=x.device)
+    assert out.dtype == x.dtype and out.is_contiguous() and tuple(out.shape[:3]) == (n, oh, ow) and out.shape[3] >= c_off + c
+    _call(_POOL[x.dtype], 0.0, _ptr(x), n, h, w, c, pitch, k, s, p, mode, _ptr(out), out.shape[3], c_off, _stream())
     return out
 
 
 def global_avg_pool(x):
-    """adaptive_avg_pool2d(x, 1).flatten(1): NHWC bf16 -> fp32 [n, C]."""
+    """adaptive_avg_pool2d(x, 1).flatten(1): NHWC bf16 or fp32 -> fp32 [n, C]."""
     n, h, w, c, pitch = _nhwc(x)
     out = torch.empty((n, c), dtype=torch.float32, device=x.device)
-    _call("ladi_pool2d_bf16", 0.0, _ptr(x), n, h, w, c, pitch, 0, 0, 0, POOL_GLOBAL_AVG_F32, _ptr(out), c, 0, _stream())
+    _call(_POOL[x.dtype], 0.0, _ptr(x), n, h, w, c, pitch, 0, 0, 0, POOL_GLOBAL_AVG_F32, _ptr(out), c, 0, _stream())
     return out
 
 
 def lpips_layer_(fa, fb, lin, acc):
-    """acc[b] += spatial mean of lin . (unit(fa) - unit(fb))^2 for NHWC bf16 feature pairs of equal shape and pitch."""
+    """acc[b] += spatial mean of lin . (unit(fa) - unit(fb))^2 for NHWC bf16 or fp32 feature pairs of equal shape, dtype and pitch."""
     n, h, w, c, pitch = _nhwc(fa)
-    assert _nhwc(fb) == (n, h, w, c, pitch) and lin.dtype == torch.float32 and lin.numel() == c and lin.is_contiguous()
+    assert fb.dtype == fa.dtype and _nhwc(fb) == (n, h, w, c, pitch) and lin.dtype == torch.float32 and lin.numel() == c and lin.is_contiguous()
     assert acc.dtype == torch.float32 and acc.numel() == n and acc.is_contiguous()
-    _call("ladi_lpips_layer", 0.0, _ptr(fa), _ptr(fb), n, h, w, c, pitch, _ptr(lin), _ptr(acc), _stream())
+    _call(_LPIPS[fa.dtype], 0.0, _ptr(fa), _ptr(fb), n, h, w, c, pitch, _ptr(lin), _ptr(acc), _stream())
     return acc
+
+
+def gemm_tf32(a, weight, n_out, out, c_off=0, bias=None, relu=False):
+    """out[:, c_off:c_off + n_out] = relu?(a @ weight[:n_out, :K]^T + bias) on TF32 tensor cores (operands rounded to nearest TF32, fp32
+    accumulation).  a: fp32 [M, K] (row-strided view fine), weight: fp32 [n_out, K'] with K' >= K (zero columns past the true reduction
+    length), out: fp32 [M, pitch] with a contiguous last dimension."""
+    assert a.dtype == weight.dtype == out.dtype == torch.float32 and a.dim() == weight.dim() == out.dim() == 2
+    assert a.stride(1) == weight.stride(1) == out.stride(1) == 1 and weight.shape[0] == n_out and out.shape[0] == a.shape[0]
+    assert out.shape[1] >= c_off + n_out and (bias is None or (bias.dtype == torch.float32 and bias.is_contiguous()))
+    m, k = a.shape
+    _call("ladi_gemm_tf32", 2.0 * m * k * n_out, _ptr(a), m, k, a.stride(0), _ptr(weight), n_out, weight.stride(0), _ptr(bias), int(relu),
+          _ptr(out), out.stride(0), c_off, _stream(), tag=f"tf32 M={m} N={n_out} K={k}")
+    return out
 
 
 def ssim(x, y):

@@ -1,8 +1,9 @@
 """Throughput of the metric networks on the engine: FID Inception-v3 images/s (299 x 299, the FID / KID path), LPIPS AlexNet pairs/s and
-SSIM pairs/s (512 x 384), at batch 32 and 64, with seeded random weights (the speed does not depend on the weight values).  Prints one
-JSON line per measurement with the card's name and power limit.  Needs a CUDA device; writes nothing.
+SSIM pairs/s (512 x 384), at batch 32 and 64, with seeded random weights (the speed does not depend on the weight values), with the
+networks in `--precision` bf16 (default) or tf32.  Prints one JSON line per measurement with the card's name and power limit.  Needs a
+CUDA device; writes nothing.
 
-    python tools/bench_metrics.py [--iters 10] [--warmup 3]
+    python tools/bench_metrics.py [--iters 10] [--warmup 3] [--precision bf16|tf32]
 """
 import argparse
 import json
@@ -41,13 +42,14 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--precision", choices=["bf16", "tf32"], default="bf16")
     a = ap.parse_args()
     from ladi_vton_b200.metrics import FIDInceptionV3, LPIPSAlex, random_state_dict, ssim
     dev = torch.device("cuda:0")
     name, limit = card()
-    inc = FIDInceptionV3()
+    inc = FIDInceptionV3(a.precision)
     inc.load_state_dict(random_state_dict(inc.param_shapes(), 0)).to(dev)
-    lp = LPIPSAlex()
+    lp = LPIPSAlex(a.precision)
     lp.load_state_dict(random_state_dict(lp.param_shapes(), 1)).to(dev)
     g = torch.Generator(device=dev).manual_seed(0)
     for batch in (32, 64):
@@ -57,7 +59,7 @@ def main():
         for what, fn, unit in (("inception_fid", lambda: inc(px), "images/s"), ("lpips_alex", lambda: lp(x, y), "pairs/s"),
                                ("ssim", lambda: ssim(x, y), "pairs/s")):
             s = timed(fn, a.iters, a.warmup)
-            print(json.dumps(dict(metric=what, batch=batch, seconds_per_batch=round(s, 6), rate=round(batch / s, 1), unit=unit, gpu=name,
+            print(json.dumps(dict(metric=what, precision=a.precision, batch=batch, seconds_per_batch=round(s, 6), rate=round(batch / s, 1), unit=unit, gpu=name,
                                   power_limit=limit)))
 
 
