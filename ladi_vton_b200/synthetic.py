@@ -30,6 +30,12 @@ def emasc_param_shapes(cin, cout, kernel_size=3, type="nonlinear"):
     return S
 
 
+def is_norm_key(k):
+    """True for the weight / bias of a GroupNorm or LayerNorm (UNet, VAE, CLIP and inversion-adapter key names)."""
+    leaf = k.rsplit(".", 1)[0].rsplit(".", 1)[-1]
+    return leaf.startswith("norm") or leaf in ("group_norm", "conv_norm_out", "layer_norm1", "layer_norm2", "post_layernorm", "final_layer_norm", "pre_layrnorm")
+
+
 def random_state_dict(shapes, seed, device="cpu", fast=False):
     """PyTorch-default-like init (U(-1/sqrt(fan_in), 1/sqrt(fan_in)) for conv/linear weights and biases, ones/zeros for
     norms), drawn in key order from one seeded generator on `device` (CPU draws are reproducible across machines and are
@@ -40,9 +46,7 @@ def random_state_dict(shapes, seed, device="cpu", fast=False):
     block = torch.empty(1 << 22, device=device).uniform_(-1.0, 1.0, generator=g) if fast else None
     for k, shp in shapes.items():
         base = k.rsplit(".", 1)[0]
-        leaf = base.rsplit(".", 1)[-1]
-        is_norm = leaf.startswith("norm") or leaf in ("group_norm", "conv_norm_out", "layer_norm1", "layer_norm2", "post_layernorm", "final_layer_norm", "pre_layrnorm")
-        if is_norm:
+        if is_norm_key(k):
             sd[k] = torch.ones(shp, device=device) if k.endswith("weight") else torch.zeros(shp, device=device)
             continue
         if k.endswith("weight"):
