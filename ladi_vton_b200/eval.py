@@ -21,6 +21,8 @@ What differs, because the target boxes have no network (the reference downloads 
     writes;
   * `--allow_tf32`, `--enable_xformers_memory_efficient_attention` are accepted: the engine always computes in bf16 and its attention is
     already fused.
+`generate_images_inversion_adapter` (src/utils/image_from_pipe.py:139-218, the inversion-adapter trainer's validation) is here too; its CLI
+is `python -m ladi_vton_b200.eval_inversion_adapter`.
 Scoring on the engine (instead of `--compute_metrics`, which runs the reference's own val_metrics.py from `--reference_src`):
 `python -m ladi_vton_b200.val_metrics --gen_folder <output_dir>/<save_name>_<test_order> --test_order <order> --dataset ... --metrics_weights_dir W`.
 """
@@ -104,15 +106,20 @@ def check_args(args):
             raise ValueError("VitonHD dataroot must be provided")
         if args.dataset == "dresscode" and args.dresscode_dataroot is None:
             raise ValueError("DressCode dataroot must be provided")
-    if args.pretrained_model_name_or_path == SD15_INPAINT or _text_width(args.pretrained_model_name_or_path) not in (None, 1024):
-        raise NotImplementedError(f"{args.pretrained_model_name_or_path}: the Stable Diffusion 1.5 inpainting base (CLIP ViT-L/14, 768-wide text "
-                                  "states, attention heads 40/80/160 wide) is not built; this engine runs the SD-2 inpainting base "
-                                  f"({SD2_INPAINT})")
+    check_base_model(args.pretrained_model_name_or_path)
     if not args.random_init:
         if args.emasc_type != 'none' and args.emasc_dir is None:
             raise ValueError("No EMASC checkpoint found. Make sure to specify --emasc_dir")
         if args.text_usage == 'inversion_adapter' and args.inversion_adapter_dir is None:
             raise ValueError("No inversion adapter checkpoint found. Make sure to specify --inversion_adapter_dir")
+
+
+def check_base_model(path):
+    """The one base model that is built: SD-2 inpainting (by name, or a local folder with a 1024-wide text encoder)."""
+    if path == SD15_INPAINT or _text_width(path) not in (None, 1024):
+        raise NotImplementedError(f"{path}: the Stable Diffusion 1.5 inpainting base (CLIP ViT-L/14, 768-wide text "
+                                  "states, attention heads 40/80/160 wide) is not built; this engine runs the SD-2 inpainting base "
+                                  f"({SD2_INPAINT})")
 
 
 def _text_width(folder):
@@ -144,18 +151,44 @@ def build_models(args, device):
     """src/eval.py:158-277 -> dict(scheduler, text_encoder, vae, tokenizer, unet, emasc, inversion_adapter, vision_encoder); emasc is None
     with --emasc_type none, inversion_adapter / vision_encoder are None unless --text_usage inversion_adapter (vision_encoder also with
     --use_clip_cloth_features, :273-275).  Every module is an engine object already on `device`."""
-    from . import AutoencoderKL, CLIPTextModel, CLIPVisionModelWithProjection, DDIMScheduler, EMASC, InversionAdapter, UNet2DConditionModel
-    from . import synthetic as S
-    load = lambda path: torch.load(path, map_location="cpu")  # noqa: E731
-    rnd = lambda mod, seed: mod.load_state_dict(S.random_state_dict(mod.param_shapes(), seed, device="cuda", fast=True))  # noqa: E731
-    m = dict(scheduler=DDIMScheduler())
+    from . import EMASC, UNet2DConditionModel
+    m = base_models(args)
     unet = UNet2DConditionModel(in_channels=27 if args.cloth_input_type == "none" else 31)  # :172
     if args.random_init:
-        from .unet import unet_param_shapes
-        from .vae import vae_param_shapes
-        m["text_encoder"] = rnd(CLIPTextModel(), args.seed + 10)
+        m["unet"] = _random_init(unet, args.seed)
+    else:
+        m["unet"] = unet.load_state_dict(_load(checkpoint_path(args.unet_dir, args.unet_name, "unet")))
+    m["emasc"] = None
+    if args.emasc_type != 'none':  # :198-226
+        em = EMASC(EMASC_IN, EMASC_OUT, kernel_size=args.emasc_kernel, padding=args.emasc_padding, stride=1, type=args.emasc_type)
+        m["emasc"] = _random_init(em, args.seed + 2) if args.random_init else em.load_state_dict(_load(checkpoint_path(args.emasc_dir, args.emasc_name, "emasc")))
+    m["inversion_adapter"] = m["vision_encoder"] = None
+    if args.text_usage == 'inversion_adapter':  # :240-278
+        m["inversion_adapter"], m["vision_encoder"] = adapter_models(args, m["text_encoder"])
+    for k, v in m.items():
+        if v is not None and hasattr(v, "to") and k not in ("scheduler", "tokenizer"):
+            v.to(device)
+    return m
+
+
+def _load(path):
+    return torch.load(path, map_location="cpu")
+
+
+def _random_init(mod, seed):
+    from . import synthetic as S
+    return mod.load_state_dict(S.random_state_dict(mod.param_shapes(), seed, device="cuda", fast=True))
+
+
+def base_models(args):
+    """The parts of the SD-2 inpainting base every validation runs (src/eval.py:158-163): dict(scheduler, text_encoder, vae, tokenizer)
+    from `--pretrained_model_name_or_path`, or seeded random weights (and the stand-in tokenizer when no tokenizer files are there)."""
+    from . import AutoencoderKL, CLIPTextModel, DDIMScheduler, synthetic as S
+    from .vae import vae_param_shapes
+    m = dict(scheduler=DDIMScheduler())
+    if args.random_init:
+        m["text_encoder"] = _random_init(CLIPTextModel(), args.seed + 10)
         m["vae"] = AutoencoderKL().load_state_dict(S.random_state_dict(vae_param_shapes({}), args.seed + 1, device="cuda", fast=True))
-        m["unet"] = unet.load_state_dict(S.random_state_dict(unet_param_shapes(dict(unet.config)), args.seed, device="cuda", fast=True))
         m["tokenizer"] = _try_tokenizer(args) or StandInTokenizer()
     else:
         root = args.pretrained_model_name_or_path
@@ -164,28 +197,42 @@ def build_models(args, device):
         m["tokenizer"] = _try_tokenizer(args)
         if m["tokenizer"] is None:
             raise FileNotFoundError(f"no tokenizer files under {root}/tokenizer")
-        m["unet"] = unet.load_state_dict(load(checkpoint_path(args.unet_dir, args.unet_name, "unet")))
-    m["emasc"] = None
-    if args.emasc_type != 'none':  # :198-226
-        em = EMASC(EMASC_IN, EMASC_OUT, kernel_size=args.emasc_kernel, padding=args.emasc_padding, stride=1, type=args.emasc_type)
-        m["emasc"] = rnd(em, args.seed + 2) if args.random_init else em.load_state_dict(load(checkpoint_path(args.emasc_dir, args.emasc_name, "emasc")))
-    m["inversion_adapter"] = m["vision_encoder"] = None
-    if args.text_usage == 'inversion_adapter':  # :240-278
-        vis = CLIPVisionModelWithProjection()
-        ia = InversionAdapter(input_dim=vis.config.hidden_size, hidden_dim=vis.config.hidden_size * 4,
-                              output_dim=m["text_encoder"].config.hidden_size * args.num_vstar, num_encoder_layers=args.num_encoder_layers,
-                              config=vis.config)
-        if args.random_init:
-            m["inversion_adapter"] = rnd(ia, args.seed + 12)
-        else:
-            m["inversion_adapter"] = ia.load_state_dict(load(checkpoint_path(args.inversion_adapter_dir, args.inversion_adapter_name, "inversion_adapter")))
-        if not args.use_clip_cloth_features:
-            m["vision_encoder"] = (rnd(vis, args.seed + 11) if args.random_init
-                                   else vis.load_state_dict(_load_folder_state_dict(args.vision_model_name_or_path), strict=False))
-    for k, v in m.items():
-        if v is not None and hasattr(v, "to") and k not in ("scheduler", "tokenizer"):
-            v.to(device)
     return m
+
+
+def adapter_models(args, text_encoder):
+    """src/eval.py:240-278 (and src/train_inversion_adapter.py:230-260): the inversion adapter with `--num_encoder_layers` layers from
+    `--inversion_adapter_dir` / `--inversion_adapter_name`, and the CLIP vision tower (None with --use_clip_cloth_features)."""
+    from . import CLIPVisionModelWithProjection, InversionAdapter
+    vis = CLIPVisionModelWithProjection()
+    ia = InversionAdapter(input_dim=vis.config.hidden_size, hidden_dim=vis.config.hidden_size * 4,
+                          output_dim=text_encoder.config.hidden_size * args.num_vstar, num_encoder_layers=args.num_encoder_layers,
+                          config=vis.config)
+    if args.random_init:
+        ia = _random_init(ia, args.seed + 12)
+    else:
+        ia = ia.load_state_dict(_load(checkpoint_path(args.inversion_adapter_dir, args.inversion_adapter_name, "inversion_adapter")))
+    vision = None
+    if not args.use_clip_cloth_features:
+        vision = (_random_init(vis, args.seed + 11) if args.random_init
+                  else vis.load_state_dict(_load_folder_state_dict(args.vision_model_name_or_path), strict=False))
+    return ia, vision
+
+
+def _pseudo_word_states(pipe, inversion_adapter, batch, vision_encoder, processor, num_vstar):
+    """image_from_pipe.py:62-83 (and :160-190): CLIP features of the cloth (the batch's `clip_cloth_features` when present) -> inversion
+    adapter -> the category prompt with `num_vstar` pseudo-words -> text encoder states."""
+    from . import encode_text_word_embedding
+    device = pipe.device
+    clip_cloth_features = batch.get("clip_cloth_features")
+    if clip_cloth_features is None:
+        clip_cloth_features = vision_encoder(clip_pixel_values(batch["cloth"], device, processor)).last_hidden_state
+    word_embeddings = inversion_adapter(clip_cloth_features.to(device))
+    word_embeddings = word_embeddings.reshape((word_embeddings.shape[0], num_vstar, -1))
+    tok = pipe.tokenizer
+    tokenized_text = tok(prompts_for(batch["category"], num_vstar), max_length=tok.model_max_length, padding="max_length", truncation=True,
+                         return_tensors="pt").input_ids
+    return encode_text_word_embedding(pipe.text_encoder, tokenized_text, word_embeddings, num_vstar).last_hidden_state
 
 
 @torch.no_grad()
@@ -193,7 +240,6 @@ def eval_batch(pipe, inversion_adapter, batch, text_usage, vision_encoder, proce
                num_inference_steps, guidance_scale):
     """The loop body of src/utils/image_from_pipe.py:42-117 -> list of PIL images.  `warped_cloth` is the dataset's (the warping module
     does not run here); the CLIP features are the batch's `clip_cloth_features` when present, else CLIP preprocessing + the vision tower."""
-    from . import encode_text_word_embedding
     model_img = batch.get("image")
     mask_img = batch.get("inpaint_mask")
     if mask_img is not None:
@@ -204,16 +250,7 @@ def eval_batch(pipe, inversion_adapter, batch, text_usage, vision_encoder, proce
     elif text_usage == "none":
         prompts = [""] * len(batch["captions"])
     elif text_usage == "inversion_adapter":
-        device = pipe.device
-        clip_cloth_features = batch.get("clip_cloth_features")
-        if clip_cloth_features is None:
-            clip_cloth_features = vision_encoder(clip_pixel_values(batch["cloth"], device, processor)).last_hidden_state
-        word_embeddings = inversion_adapter(clip_cloth_features.to(device))
-        word_embeddings = word_embeddings.reshape((word_embeddings.shape[0], num_vstar, -1))
-        tok = pipe.tokenizer
-        tokenized_text = tok(prompts_for(batch["category"], num_vstar), max_length=tok.model_max_length, padding="max_length", truncation=True,
-                             return_tensors="pt").input_ids
-        encoder_hidden_states = encode_text_word_embedding(pipe.text_encoder, tokenized_text, word_embeddings, num_vstar).last_hidden_state
+        encoder_hidden_states = _pseudo_word_states(pipe, inversion_adapter, batch, vision_encoder, processor, num_vstar)
     else:
         raise ValueError(f"Unknown text usage {text_usage}")
     kw = dict(image=model_img, mask_image=mask_img, pose_map=pose_map, warped_cloth=warped_cloth, height=512, width=384,
@@ -237,6 +274,32 @@ def generate_images_from_tryon_pipe(pipe, inversion_adapter, test_dataloader, ou
     for batch in test_dataloader:
         images = eval_batch(pipe, inversion_adapter, batch, text_usage, vision_encoder, processor, cloth_input_type, cloth_cond_rate, num_vstar,
                             generator, num_inference_steps, guidance_scale)
+        written += save_images(images, batch["category"], batch["im_name"], save_path, use_png)
+    return written
+
+
+@torch.no_grad()
+def adapter_val_batch(pipe, inversion_adapter, vision_encoder, processor, batch, num_vstar, generator, num_inference_steps, guidance_scale):
+    """The loop body of src/utils/image_from_pipe.py:154-203 -> list of PIL images: pseudo-word text states from the cloth, then the
+    inpainting pipeline on the person image and its inpainting mask at 512x384, one image per prompt."""
+    encoder_hidden_states = _pseudo_word_states(pipe, inversion_adapter, batch, vision_encoder, processor, num_vstar)
+    return pipe(image=batch["image"], mask_image=batch["inpaint_mask"].type(torch.float32), prompt_embeds=encoder_hidden_states, height=512,
+                width=384, guidance_scale=guidance_scale, num_images_per_prompt=1, generator=generator,
+                num_inference_steps=num_inference_steps).images
+
+
+@torch.no_grad()
+def generate_images_inversion_adapter(pipe, inversion_adapter, vision_encoder, processor, test_dataloader, output_dir, order: str,
+                                      save_name: str, num_vstar=1, seed=1234, num_inference_steps=50, guidance_scale=7.5, use_png=False):
+    """src/utils/image_from_pipe.py:139-218 (same signature): every batch of `test_dataloader` through `adapter_val_batch` with one CUDA
+    generator seeded once, images written to `<output_dir>/<save_name>_<order>/<category>/<im_name>`.  Returns the written paths."""
+    save_path = os.path.join(output_dir, f"{save_name}_{order}")
+    os.makedirs(save_path, exist_ok=True)
+    generator = torch.Generator("cuda").manual_seed(seed)
+    written = []
+    for batch in test_dataloader:
+        images = adapter_val_batch(pipe, inversion_adapter, vision_encoder, processor, batch, num_vstar, generator, num_inference_steps,
+                                   guidance_scale)
         written += save_images(images, batch["category"], batch["im_name"], save_path, use_png)
     return written
 

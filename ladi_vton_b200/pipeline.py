@@ -1,5 +1,7 @@
 """`StableDiffusionTryOnePipeline` -- same constructor, `.to()`, `__call__` signature/defaults/return types and error
-behaviour as the reference's src/vto_pipelines/tryon_pipe.py:27-765, with the body re-built H100-first:
+behaviour as the reference's src/vto_pipelines/tryon_pipe.py:27-765 -- and `StableDiffusionInpaintPipeline`, the diffusers 0.14
+inpainting pipeline the reference validates inversion adapters with (src/train_inversion_adapter.py:546-556).  Both run one body
+(`_EnginePipeline._generate`) that differs only in the conditioning layout of the UNet input, re-built H100-first:
 
   * all model arithmetic runs in the hand-written sm_90a kernels (ops.py) -- NHWC bf16 activations, fp32 latents;
   * step-invariant work is hoisted out of the loop (27 of the 31 UNet input channels, text K/V, time-embedding tables);
@@ -46,13 +48,16 @@ class _Session:
     UNet input assembly, text K/V), `loop` (all N denoising steps; or `step`, one step replayed N times, when something has to happen on the
     host between steps: eta > 0, cloth_cond_rate < 1, a callback) and `post` (VAE decode with the EMASC skips + image conversion)."""
 
-    def __init__(self, B, Bp, h, w, H, W, in_pitch, n_pose, ctx_shape, kv_total, device):
+    def __init__(self, B, Bp, h, w, H, W, in_pitch, n_pose, ctx_shape, kv_total, device, Bi=None):
+        """`Bi`: the number of images / masks passed (default B); `pre` tiles them to the effective batch B."""
         f32 = dict(dtype=torch.float32, device=device)
-        self.image = torch.zeros((B, 3, H, W), **f32)
-        self.mask = torch.zeros((B, 1, H, W), **f32)
+        Bi = Bi or B
+        self.image = torch.zeros((Bi, 3, H, W), **f32)
+        self.mask = torch.zeros((Bi, 1, H, W), **f32)
         self.pose = torch.zeros((B, n_pose, H, W), **f32)
         self.cloth = torch.zeros((B, 3, H, W), **f32)
-        self.noise = [torch.zeros((B, 4, h, w), **f32) for _ in range(3)]  # cloth posterior, initial latents, masked-image posterior
+        # cloth posterior, initial latents, masked-image posterior (one draw per image passed)
+        self.noise = [torch.zeros((B, 4, h, w), **f32), torch.zeros((B, 4, h, w), **f32), torch.zeros((Bi, 4, h, w), **f32)]
         self.step_noise = torch.zeros((B, 4, h, w), **f32)                 # eta > 0: DDIM variance noise of the current step
         self.ctx = torch.zeros(ctx_shape, dtype=torch.bfloat16, device=device)
         self.ctx_kv = torch.zeros((ctx_shape[0], ctx_shape[1], kv_total), dtype=torch.bfloat16, device=device)
@@ -70,7 +75,10 @@ class _Session:
         self.step_nodes = self.pre_nodes = self.post_nodes = self.loop_nodes = 0
 
 
-class StableDiffusionTryOnePipeline:
+class _EnginePipeline:
+    """What the try-on and the inpainting pipeline share: constructor state, `.to()`, prompt encoding, mask / image preparation, the
+    captured `pre` / `step` / `post` pieces and the call body `_generate`, parameterised by the UNet input layout `lay`
+    (latents4 | mask1 | masked4 [| pose | cloth4])."""
     _optional_components = ["safety_checker"]
 
     def __init__(self, vae, text_encoder, tokenizer, unet, scheduler, safety_checker=None, feature_extractor=None,
@@ -194,11 +202,9 @@ class StableDiffusionTryOnePipeline:
             mask = np.concatenate([m[None, None, :] for m in mask], axis=0).astype(np.float32)
         return image, torch.from_numpy(np.ascontiguousarray(mask))
 
-    def _prepare_mask_and_image(self, image, mask, flags):
-        """diffusers prepare_mask_and_masked_image (called at tryon_pipe.py:630): shape normalisation, the [-1,1] / [0,1] range checks and
-        the IN-PLACE binarisation of the caller's mask at 0.5.  Device tensors: one kernel, the range flags are read back with the
-        result (no host sync before the work is queued); host tensors: checked on the host, raising at once like the reference.
-        `image * (mask < 0.5)` itself is fused into the layout kernel (ops.nchw_to_nhwc gate)."""
+    def _as_tensors(self, image, mask):
+        """The shape half of diffusers prepare_mask_and_masked_image: PIL / ndarray inputs converted, both made 4-D (views of the
+        caller's tensors, so the binarisation below still writes the caller's mask), batch and size checked."""
         if not isinstance(image, torch.Tensor) or not isinstance(mask, torch.Tensor):
             if isinstance(image, torch.Tensor) or isinstance(mask, torch.Tensor):
                 raise TypeError("`image` and `mask_image` must both be torch tensors or both PIL images / arrays")
@@ -214,6 +220,14 @@ class StableDiffusionTryOnePipeline:
         assert image.ndim == 4 and mask.ndim == 4, "Image and Mask must have 4 dimensions"
         assert image.shape[-2:] == mask.shape[-2:], "Image and Mask must have the same spatial dimensions"
         assert image.shape[0] == mask.shape[0], "Image and Mask must have the same batch size"
+        return image, mask
+
+    def _prepare_mask_and_image(self, image, mask, flags):
+        """diffusers prepare_mask_and_masked_image (called at tryon_pipe.py:630): shape normalisation, the [-1,1] / [0,1] range checks and
+        the IN-PLACE binarisation of the caller's mask at 0.5.  Device tensors: one kernel, the range flags are read back with the
+        result (no host sync before the work is queued); host tensors: checked on the host, raising at once like the reference.
+        `image * (mask < 0.5)` itself is fused into the layout kernel (ops.nchw_to_nhwc gate)."""
+        image, mask = self._as_tensors(image, mask)
         fast = all(t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() for t in (image, mask))
         if fast:
             ops.check_binarise_(image, mask, flags)
@@ -245,9 +259,9 @@ class StableDiffusionTryOnePipeline:
             mom, _ = self.vae.encode_nhwc(s.cloth)
             ops.nchw_to_nhwc(ops.posterior_sample(mom, s.noise[0], sf), cond, c_off=lay["c_cloth"])
         s.latents.copy_(s.noise[1])  # 6. latents (RNG draw #2, already times init_noise_sigma)
-        # 7. masked image -> latents + encoder skips (RNG draw #3); EMASC with mask_features fused
-        H, W = s.image.shape[2], s.image.shape[3]
-        masked = torch.zeros((B, H, W, 8), dtype=torch.bfloat16, device=self.device)
+        # 7. masked image -> latents + encoder skips (RNG draw #3, one per image passed); EMASC with mask_features fused
+        Bi, H, W = s.image.shape[0], s.image.shape[2], s.image.shape[3]
+        masked = torch.zeros((Bi, H, W, 8), dtype=torch.bfloat16, device=self.device)
         ops.nchw_to_nhwc(s.image, masked, gate=s.mask)  # image * (mask < 0.5)
         mom, feats = self.vae.encode_nhwc(masked, nhwc=True)
         masked_lat = ops.posterior_sample(mom, s.noise[2], sf)
@@ -257,8 +271,9 @@ class StableDiffusionTryOnePipeline:
             inv = [ops.inv_mask_rows(s.mask, H // f.shape[1]) for f in sel]  # data_utils.py:9-14 (chained nearest == direct)
             s.inter = self.emasc(sel, inv)  # :684-685
         for half in ((s.unet_in[:B], s.unet_in[B:]) if cfg else (s.unet_in,)):  # :482-485
-            ops.nchw_to_nhwc(s.mask, half, c_off=lay["c_mask"], f=vsf)  # nearest /8 (:434-436)
-            ops.nchw_to_nhwc(masked_lat, half, c_off=lay["c_masked"])
+            for r in range(0, B, Bi):  # :462-477: mask and masked latents repeated to the effective batch, rows [a, b, a, b]
+                ops.nchw_to_nhwc(s.mask, half[r:r + Bi], c_off=lay["c_mask"], f=vsf)  # nearest /8 (:434-436)
+                ops.nchw_to_nhwc(masked_lat, half[r:r + Bi], c_off=lay["c_masked"])
             ops.nchw_to_nhwc(s.latents, half, c_off=0)
         self.unet.plan_context(s.ctx, out=s.ctx_kv)  # step-invariant: text K/V of all 16 cross-attention layers
         s.step.zero_()
@@ -296,59 +311,44 @@ class StableDiffusionTryOnePipeline:
         getattr(s, g_attr).replay()
         lib.launches += getattr(s, n_attr)
 
-    @torch.no_grad()
-    def __call__(self, image, mask_image, pose_map, warped_cloth, prompt=None, height=None, width=None,
-                 num_inference_steps: int = 50, guidance_scale: float = 7.5, negative_prompt=None, num_images_per_prompt=1,
-                 eta: float = 0.0, prompt_embeds=None, negative_prompt_embeds=None, generator=None, latents=None,
-                 output_type="pil", return_dict: bool = True, callback=None, callback_steps=1, cloth_cond_rate: float = 1.0,
-                 no_pose: bool = False, cloth_input_type: str = "warped", noise=None):
-        """Same arguments as the reference `__call__` (tryon_pipe.py:495-520).  Extensions: output_type="pt" returns the
-        device tensor; `noise=(cloth, latents, masked)` supplies the three RNG draws explicitly (batch-sharded runs slice
-        one full-batch draw, distributed.draw_noise)."""
+    def _generate(self, lay, Bi, image, mask_image, pose_map, warped_cloth, prompt, height, width, num_inference_steps, guidance_scale,
+                  negative_prompt, num_images_per_prompt, eta, prompt_embeds, negative_prompt_embeds, generator, latents, output_type,
+                  return_dict, callback, callback_steps, cloth_cond_rate=1.0, noise=None):
+        """The call body of both pipelines (tryon_pipe.py:578-765) for the UNet input layout `lay` (c_mask, c_masked, c_pose, c_cloth,
+        no_pose, cloth).  `Bi`: the number of images / masks passed, tiled to the effective batch as prepare_mask_latents does
+        (None: the images already have the effective batch)."""
         dev = self.device
-        if dev.type != "cuda":
-            raise RuntimeError("call .to('cuda') first: ladi_vton_b200 has no CPU path")
-        height = height or self.unet.config.sample_size * self.vae_scale_factor
-        width = width or self.unet.config.sample_size * self.vae_scale_factor
-        self.check_inputs(prompt, height, width, callback_steps, negative_prompt, prompt_embeds, negative_prompt_embeds)
-        if image is None:
-            raise ValueError("`image` input cannot be undefined.")
-        if mask_image is None:
-            raise ValueError("`mask_image` input cannot be undefined.")
-        if cloth_input_type not in ("warped", "none"):
-            raise ValueError(f"Invalid cloth_input_type {cloth_input_type}")
-        if num_images_per_prompt != 1:
-            # the reference accepts the argument but its own body then concatenates [B*num, ...] latents with [B, ...] pose / cloth
-            # tensors (tryon_pipe.py:702-726) and fails inside torch.cat; say so instead of failing somewhere in a kernel wrapper
-            raise ValueError("num_images_per_prompt != 1 is not supported by the try-on pipeline: pose_map / warped_cloth are not repeated "
-                             "to the effective batch (the reference fails in torch.cat at tryon_pipe.py:724); repeat the inputs instead")
         if prompt is not None:
             batch_size = 1 if isinstance(prompt, str) else len(prompt)
         else:
             batch_size = prompt_embeds.shape[0]
-        cfg = guidance_scale > 1.0
-        ctx = self._encode_prompt(prompt, dev, num_images_per_prompt, cfg, negative_prompt, prompt_embeds, negative_prompt_embeds)
         B = batch_size * num_images_per_prompt
-        Bp = 2 * B if cfg else B
-        vsf = self.vae_scale_factor
-        h, w = height // vsf, width // vsf
         if isinstance(generator, (list, tuple)) and len(generator) != 1 and len(generator) != B:  # prepare_latents :412-416
             raise ValueError(f"You have passed a list of generators of length {len(generator)}, but requested an effective batch"
                              f" size of {B}. Make sure the batch size matches the length of the generators.")
+        Bi = Bi or B
+        _check_tiling(Bi, Bi, B)
+        if isinstance(generator, (list, tuple)) and len(generator) != 1 and Bi < B:
+            # prepare_mask_latents :442-446 encodes masked_image[i] with generator[i] for every i < B: past the end of the images passed
+            raise ValueError(f"a list of {len(generator)} generators draws one masked-image latent per sample, but only {Bi} images were"
+                             f" passed for an effective batch of {B}: pass {B} images, or one generator")
+        cfg = guidance_scale > 1.0
+        ctx = self._encode_prompt(prompt, dev, num_images_per_prompt, cfg, negative_prompt, prompt_embeds, negative_prompt_embeds)
+        Bp = 2 * B if cfg else B
+        vsf = self.vae_scale_factor
+        h, w = height // vsf, width // vsf
 
         # ---- session (static buffers + graphs) for this shape / conditioning layout
-        n_pose = pose_map.shape[1]
-        cin = self.unet.config.in_channels
-        lay = dict(B=B, cfg=cfg, no_pose=bool(no_pose), cloth=cloth_input_type == "warped", c_mask=4, c_masked=5, c_pose=9, c_cloth=9 + n_pose)
-        assert cin == lay["c_cloth"] + (4 if lay["cloth"] else 0), "UNet in_channels does not match the conditioning"
+        n_pose = lay["c_cloth"] - lay["c_pose"]
+        lay = dict(lay, B=B, cfg=cfg)
         gens = (self.unet.pack_gen, self.vae.pack_gen, self.emasc.pack_gen if self.emasc else 0)
         if gens != self._pack_gens:  # weights were re-packed: every captured graph points at freed memory
             self._sessions.clear()
             self._pack_gens = gens
-        key = (B, Bp, h, w, n_pose, lay["no_pose"], lay["cloth"], bool(self.emasc), tuple(ctx.shape[1:]))
+        key = (B, Bp, Bi, h, w, n_pose, lay["no_pose"], lay["cloth"], bool(self.emasc), tuple(ctx.shape[1:]))
         s = self._sessions.get(key)
         if s is None:
-            s = self._sessions[key] = _Session(B, Bp, h, w, height, width, self.unet.in_pitch, n_pose, tuple(ctx.shape), self.unet.kv_total, dev)
+            s = self._sessions[key] = _Session(B, Bp, h, w, height, width, self.unet.in_pitch, n_pose, tuple(ctx.shape), self.unet.kv_total, dev, Bi)
         use_graph = self.use_cuda_graph and s.calls > 0  # the first call of a shape runs eagerly: lazy kernel attributes, allocations
 
         # 4. mask / image validation + in-place binarisation (flags read back with the result), inputs -> static buffers
@@ -370,7 +370,7 @@ class StableDiffusionTryOnePipeline:
         if latents is None:
             latents = noise[1] if noise is not None else _randn((B, 4, h, w), generator, dev)
         s.noise[1].copy_(latents.to(dev, torch.float32) * self.scheduler.init_noise_sigma, non_blocking=True)
-        s.noise[2].copy_(noise[2] if noise is not None else _randn((B, 4, h, w), generator, dev), non_blocking=True)
+        s.noise[2].copy_(noise[2] if noise is not None else _randn((Bi, 4, h, w), generator, dev), non_blocking=True)
         self._run(s, "pre", lambda: self._pre(s, lay), (self.unet.ws.buf.data_ptr() if self.unet.ws.buf is not None else 0,
                                                        self.vae.ws.buf.data_ptr() if self.vae.ws.buf is not None else 0), use_graph)
         self.unet._ctx = s.ctx_kv  # (a replayed `pre` graph did not run plan_context's Python)
@@ -435,7 +435,96 @@ class StableDiffusionTryOnePipeline:
             return (out, None)
         return StableDiffusionPipelineOutput(images=out, nsfw_content_detected=None)
 
+
     def _graph_key(self):
         # the captured step graph bakes in the addresses of the planned step table, the text K/V buffer and the GroupNorm workspace
         ws = self.unet.ws.buf
         return (self.unet._steps.data_ptr(), self.unet._ctx.data_ptr(), self.unet._steps.shape[0], ws.data_ptr() if ws is not None else 0)
+
+
+def _check_tiling(n_masks, n_images, batch_size):
+    """prepare_mask_latents (tryon_pipe.py:462-477): the masks and the masked-image latents passed are repeated to the effective batch,
+    whole copies only.  More images than samples has no repeat that fits (the reference fails in torch.cat, :724)."""
+    if n_masks < batch_size and batch_size % n_masks != 0:
+        raise ValueError("The passed mask and the required batch size don't match. Masks are supposed to be duplicated to"
+                         f" a total batch size of {batch_size}, but {n_masks} masks were passed. Make sure the number"
+                         " of masks that you pass is divisible by the total requested batch size.")
+    if n_images < batch_size and batch_size % n_images != 0:
+        raise ValueError("The passed images and the required batch size don't match. Images are supposed to be duplicated"
+                         f" to a total batch size of {batch_size}, but {n_images} images were passed."
+                         " Make sure the number of images that you pass is divisible by the total requested batch size.")
+    if max(n_masks, n_images) > batch_size:
+        raise ValueError(f"{max(n_masks, n_images)} images / masks were passed for an effective batch of {batch_size}"
+                         " (prompts x num_images_per_prompt): pass at most one image per sample")
+
+
+class StableDiffusionTryOnePipeline(_EnginePipeline):
+
+    @torch.no_grad()
+    def __call__(self, image, mask_image, pose_map, warped_cloth, prompt=None, height=None, width=None,
+                 num_inference_steps: int = 50, guidance_scale: float = 7.5, negative_prompt=None, num_images_per_prompt=1,
+                 eta: float = 0.0, prompt_embeds=None, negative_prompt_embeds=None, generator=None, latents=None,
+                 output_type="pil", return_dict: bool = True, callback=None, callback_steps=1, cloth_cond_rate: float = 1.0,
+                 no_pose: bool = False, cloth_input_type: str = "warped", noise=None):
+        """Same arguments as the reference `__call__` (tryon_pipe.py:495-520).  Extensions: output_type="pt" returns the
+        device tensor; `noise=(cloth, latents, masked)` supplies the three RNG draws explicitly (batch-sharded runs slice
+        one full-batch draw, distributed.draw_noise)."""
+        if self.device.type != "cuda":
+            raise RuntimeError("call .to('cuda') first: ladi_vton_b200 has no CPU path")
+        height = height or self.unet.config.sample_size * self.vae_scale_factor
+        width = width or self.unet.config.sample_size * self.vae_scale_factor
+        self.check_inputs(prompt, height, width, callback_steps, negative_prompt, prompt_embeds, negative_prompt_embeds)
+        if image is None:
+            raise ValueError("`image` input cannot be undefined.")
+        if mask_image is None:
+            raise ValueError("`mask_image` input cannot be undefined.")
+        if cloth_input_type not in ("warped", "none"):
+            raise ValueError(f"Invalid cloth_input_type {cloth_input_type}")
+        if num_images_per_prompt != 1:
+            # the reference accepts the argument but its own body then concatenates [B*num, ...] latents with [B, ...] pose / cloth
+            # tensors (tryon_pipe.py:702-726) and fails inside torch.cat; say so instead of failing somewhere in a kernel wrapper
+            raise ValueError("num_images_per_prompt != 1 is not supported by the try-on pipeline: pose_map / warped_cloth are not repeated "
+                             "to the effective batch (the reference fails in torch.cat at tryon_pipe.py:724); repeat the inputs instead")
+        n_pose = pose_map.shape[1]
+        lay = dict(no_pose=bool(no_pose), cloth=cloth_input_type == "warped", c_mask=4, c_masked=5, c_pose=9, c_cloth=9 + n_pose)
+        assert self.unet.config.in_channels == lay["c_cloth"] + (4 if lay["cloth"] else 0), "UNet in_channels does not match the conditioning"
+        return self._generate(lay, None, image, mask_image, pose_map, warped_cloth, prompt, height, width, num_inference_steps, guidance_scale,
+                              negative_prompt, num_images_per_prompt, eta, prompt_embeds, negative_prompt_embeds, generator, latents,
+                              output_type, return_dict, callback, callback_steps, cloth_cond_rate, noise)
+
+
+class StableDiffusionInpaintPipeline(_EnginePipeline):
+    """diffusers 0.14 `StableDiffusionInpaintPipeline` on the engine: the stock SD-2 inpainting model (9-channel UNet input
+    latents4 | mask1 | masked4), as src/train_inversion_adapter.py:546-556 builds it to validate an inversion adapter.  The same
+    body as the try-on pipeline without pose, cloth and EMASC, plus `num_images_per_prompt > 1`: prompt embeddings and initial
+    latents grouped per prompt ([a, a, b, b]), the images passed encoded once each and tiled ([a, b, a, b]).  No safety checker
+    is built: `nsfw_content_detected` is None."""
+
+    def __init__(self, vae, text_encoder, tokenizer, unet, scheduler, safety_checker=None, feature_extractor=None,
+                 requires_safety_checker: bool = True):
+        super().__init__(vae, text_encoder, tokenizer, unet, scheduler, safety_checker, feature_extractor, requires_safety_checker)
+
+    @torch.no_grad()
+    def __call__(self, prompt=None, image=None, mask_image=None, height=None, width=None, num_inference_steps: int = 50,
+                 guidance_scale: float = 7.5, negative_prompt=None, num_images_per_prompt=1, eta: float = 0.0, generator=None,
+                 latents=None, prompt_embeds=None, negative_prompt_embeds=None, output_type="pil", return_dict: bool = True,
+                 callback=None, callback_steps=1):
+        """Same arguments, defaults and return types as diffusers 0.14; output_type="pt" (extension) returns the device tensor."""
+        if self.device.type != "cuda":
+            raise RuntimeError("call .to('cuda') first: ladi_vton_b200 has no CPU path")
+        height = height or self.unet.config.sample_size * self.vae_scale_factor
+        width = width or self.unet.config.sample_size * self.vae_scale_factor
+        self.check_inputs(prompt, height, width, callback_steps, negative_prompt, prompt_embeds, negative_prompt_embeds)
+        if image is None:
+            raise ValueError("`image` input cannot be undefined.")
+        if mask_image is None:
+            raise ValueError("`mask_image` input cannot be undefined.")
+        if 4 + 1 + 4 != self.unet.config.in_channels:
+            raise ValueError(f"Incorrect configuration settings! The config of `pipeline.unet` expects {self.unet.config.in_channels} input"
+                             " channels but received `num_channels_latents`: 4 + `num_channels_mask`: 1 + `num_channels_masked_image`: 4"
+                             " = 9. Please verify the config of `pipeline.unet` or your `mask_image` or `image` input.")
+        image, mask_image = self._as_tensors(image, mask_image)
+        lay = dict(no_pose=True, cloth=False, c_mask=4, c_masked=5, c_pose=9, c_cloth=9)
+        return self._generate(lay, image.shape[0], image, mask_image, None, None, prompt, height, width, num_inference_steps, guidance_scale,
+                              negative_prompt, num_images_per_prompt, eta, prompt_embeds, negative_prompt_embeds, generator, latents,
+                              output_type, return_dict, callback, callback_steps)
