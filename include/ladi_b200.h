@@ -259,6 +259,11 @@ LADI_API int ladi_image_out(const void* x, int x_is_fp32, int n, int h, int w, i
  * tryon_pipe.py:760; round-half-to-even like numpy): NHWC uint8 [n,h,w,3], so output_type="pil" moves a quarter of the bytes to the host.
  * x_pitch >= 3.  NaN gives 0 (numpy's NaN -> uint8 cast has no defined value). */
 LADI_API int ladi_image_out_u8(const void* x, int x_is_fp32, int n, int h, int w, int x_pitch, unsigned char* out, void* stream);
+/* The EMASC trainer's reconstruction writer (src/utils/image_from_pipe.py:252-258: `(x + 1) / 2`, then torchvision.utils.save_image's
+ * `mul(255).add_(0.5).clamp_(0, 255).to(uint8)`): t = (x + 1) * 0.5, u = fl(fl(t * 255) + 0.5) with two roundings (no FMA), clamp to
+ * [0, 255], truncate.  x NHWC fp32 [n,h,w,pitch] (first 3 channels, as ladi_vae_decode_emasc writes it) -> NHWC uint8 [n,h,w,3];
+ * x_pitch >= 3.  NaN gives 0. */
+LADI_API int ladi_image_save_u8(const float* x, int n, int h, int w, int x_pitch, unsigned char* out, void* stream);
 /* Sinusoidal timestep embedding of the UNet (diffusers get_timestep_embedding, flip_sin_to_cos, the input of time_embedding.linear_1; SURVEY App. A.2)
  * for n timesteps (device fp32 [n]), written as a (hi, lo) pair of bf16 column blocks: out bf16 [n, 2*k_pad], hi at columns [0, channels),
  * lo = bf16(e - hi) at [k_pad, k_pad + channels), zeros elsewhere (k_pad = channels rounded up to 64: the K layout of the packed [W | W] weight). */

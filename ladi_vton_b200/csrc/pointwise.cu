@@ -577,6 +577,21 @@ __global__ void image_out_u8_kernel(const void* __restrict__ x, int is_f32, int6
   }
 }
 
+// The EMASC trainer's image writer (src/utils/image_from_pipe.py:252-258): `(x + 1) / 2`, then torchvision.utils.save_image's
+// `mul(255).add_(0.5).clamp_(0, 255).to(uint8)`.  Each step is its own fp32 rounding, as torch runs them: `(x + 1) * 0.5` equals the
+// division by 2 exactly, and __fmul_rn / __fadd_rn keep nvcc from contracting `t * 255 + 0.5` into one FMA, which rounds once and gives
+// another byte at near-ties.  The cast truncates.  NaN gives 0 (fmaxf picks the 0), as in image_out_u8_kernel.
+__global__ void image_save_u8_kernel(const float* __restrict__ x, int64_t npx, int x_pitch, uint8_t* __restrict__ out) {
+  ptx::pdl_wait();
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < npx * 3; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t px = i / 3;
+    const int ch = (int)(i % 3);
+    const float t = __fmul_rn(__fadd_rn(x[px * x_pitch + ch], 1.f), 0.5f);
+    const float u = fminf(fmaxf(__fadd_rn(__fmul_rn(t, 255.f), 0.5f), 0.f), 255.f);
+    out[i] = (uint8_t)__float2uint_rz(u);
+  }
+}
+
 // src/utils/posemap.py:6-35 kpoint_to_heatmap for all key-points of a batch: out[b,k,y,x] = exp(-((x-kx)^2 + (y-ky)^2) / sigma^2) / (max + eps)
 // when any coordinate of the key-point is > 0, else 0.  The maximum over the integer grid is attained at the grid point nearest to the
 // key-point (clamped into the map), so it has a closed form and the map is written in one pass.
@@ -883,6 +898,12 @@ extern "C" int ladi_check_binarise(const float* image, long long n_image, float*
 extern "C" int ladi_image_out_u8(const void* x, int x_is_fp32, int n, int h, int w, int x_pitch, unsigned char* out, void* stream) {
   LADI_CHECK(x && out && n > 0 && h > 0 && w > 0 && x_pitch >= 3, "image_out_u8: bad extent");
   LADI_CUDA(ladi_launch(image_out_u8_kernel, dim3(grid_for((int64_t)n * h * w * 3)), dim3(256), 0, STREAM, x, x_is_fp32, (int64_t)n * h * w, x_pitch, out));
+  return LADI_OK;
+}
+
+extern "C" int ladi_image_save_u8(const float* x, int n, int h, int w, int x_pitch, unsigned char* out, void* stream) {
+  LADI_CHECK(x && out && n > 0 && h > 0 && w > 0 && x_pitch >= 3, "image_save_u8: bad extent");
+  LADI_CUDA(ladi_launch(image_save_u8_kernel, dim3(grid_for((int64_t)n * h * w * 3)), dim3(256), 0, STREAM, x, (int64_t)n * h * w, x_pitch, out));
   return LADI_OK;
 }
 

@@ -22,7 +22,8 @@ What differs, because the target boxes have no network (the reference downloads 
   * `--allow_tf32`, `--enable_xformers_memory_efficient_attention` are accepted: the engine always computes in bf16 and its attention is
     already fused.
 `generate_images_inversion_adapter` (src/utils/image_from_pipe.py:139-218, the inversion-adapter trainer's validation) is here too; its CLI
-is `python -m ladi_vton_b200.eval_inversion_adapter`.
+is `python -m ladi_vton_b200.eval_inversion_adapter`, and so is `extract_save_vae_images` (src/utils/image_from_pipe.py:221-258, the EMASC
+trainer's reconstruction check), whose CLI is `python -m ladi_vton_b200.eval_emasc`.
 Scoring on the engine (instead of `--compute_metrics`, which runs the reference's own val_metrics.py from `--reference_src`):
 `python -m ladi_vton_b200.val_metrics --gen_folder <output_dir>/<save_name>_<test_order> --test_order <order> --dataset ... --metrics_weights_dir W`.
 """
@@ -301,6 +302,54 @@ def generate_images_inversion_adapter(pipe, inversion_adapter, vision_encoder, p
         images = adapter_val_batch(pipe, inversion_adapter, vision_encoder, processor, batch, num_vstar, generator, num_inference_steps,
                                    guidance_scale)
         written += save_images(images, batch["category"], batch["im_name"], save_path, use_png)
+    return written
+
+
+def write_image(u8, path):
+    """The tail of torchvision.utils.save_image for one image already quantised by its rule (ops.image_save_u8): `Image.fromarray(ndarr)
+    .save(fp)` with the format taken from the file name and no other argument.  The reference passes `quality=95`, which never reaches
+    PIL (DESIGN.md section 7), so a `.jpg` is written at PIL's default quality, as it is here."""
+    from PIL import Image
+    Image.fromarray(u8).save(path)
+
+
+@torch.no_grad()
+def vae_recon_batch(vae, emasc, batch, int_layers, emasc_type):
+    """The loop body of src/utils/image_from_pipe.py:234-249 on the device -> the decoded images, NHWC fp32 [B,H,W,4] (first 3 channels):
+    the posterior of `image`, the skips `int_layers` of `im_mask` through EMASC with `mask_features` by `inpaint_mask` fused, one
+    posterior draw from the global CUDA RNG ([B,4,h,w], as randn_tensor without a generator), and the decode with the skips.
+    With emasc_type "none": encode, sample and decode without skips (the reference's branch reads `.latent_dist` off the
+    tuple `encode` returns and cannot run; this is what it means to do, the VAE-only reconstruction)."""
+    from . import ops
+    from .vae import DiagonalGaussianDistribution
+    device = vae.device
+    image = batch["image"].to(device, torch.float32)
+    mom, _ = vae.encode_nhwc(image)
+    feats = None
+    if emasc_type != "none":
+        _, skips = vae.encode_nhwc(batch["im_mask"].to(device, torch.float32))
+        sel = [skips[i] for i in int_layers]
+        mask = batch["inpaint_mask"].to(device, torch.float32).contiguous()
+        feats = emasc(sel, [ops.inv_mask_rows(mask, image.shape[2] // f.shape[1]) for f in sel])
+    latents = DiagonalGaussianDistribution(mom, vae.config.latent_channels).sample()
+    return vae.decode_nhwc(latents, feats, list(int_layers) if feats is not None else None)
+
+
+@torch.no_grad()
+def extract_save_vae_images(vae, emasc, test_dataloader, int_layers, output_dir: str, order: str, save_name: str, emasc_type: str):
+    """src/utils/image_from_pipe.py:221-258 (same signature), the EMASC trainer's validation: every batch of `test_dataloader` through
+    `vae_recon_batch`, save_image's quantisation of `(x + 1) / 2` on the device (ops.image_save_u8), one device-to-host copy of the uint8
+    images, each written by `write_image` to `<output_dir>/<save_name>_<order>/<category>/<im_name>`.  Returns the written paths."""
+    from . import ops
+    save_path = os.path.join(output_dir, f"{save_name}_{order}")
+    os.makedirs(save_path, exist_ok=True)
+    written = []
+    for batch in test_dataloader:
+        u8 = ops.image_save_u8(vae_recon_batch(vae, emasc, batch, int_layers, emasc_type)).cpu().numpy()
+        for img, cat, name in zip(u8, batch["category"], batch["im_name"]):
+            os.makedirs(os.path.join(save_path, cat), exist_ok=True)
+            write_image(img, os.path.join(save_path, cat, name))
+            written.append(os.path.join(save_path, cat, name))
     return written
 
 

@@ -94,14 +94,15 @@ def check_base_unet(root):
                          "in_channels=9 (latents 4 + mask 1 + masked image 4); a try-on UNet is evaluated with ladi_vton_b200.eval")
 
 
-def default_save_name(args):
-    """`imgs_step_<step>` (src/train_inversion_adapter.py:562) with the step of the checkpoint file `inversion_adapter_<step>.pth`."""
+def default_save_name(args, prefix="inversion_adapter"):
+    """`imgs_step_<step>` (src/train_inversion_adapter.py:562, src/train_emasc.py:446) with the step of the checkpoint file
+    `<prefix>_<step>.pth`, found from `args.<prefix>_dir` and `args.<prefix>_name` (`latest`: the highest step)."""
     if args.random_init:
         return SAVE_NAME.format("random_init")
-    name = os.path.basename(checkpoint_path(args.inversion_adapter_dir, args.inversion_adapter_name, "inversion_adapter"))
+    name = os.path.basename(checkpoint_path(getattr(args, f"{prefix}_dir"), getattr(args, f"{prefix}_name"), prefix))
     step = os.path.splitext(name)[0].split("_")[-1]
     if not step.isdigit():
-        raise ValueError(f"{name} does not end in a training step (inversion_adapter_<step>.pth): pass --save_name")
+        raise ValueError(f"{name} does not end in a training step ({prefix}_<step>.pth): pass --save_name")
     return SAVE_NAME.format(int(step))
 
 

@@ -107,6 +107,7 @@ SIGNATURES = {
     "ladi_check_binarise": ([_P, _L, _P, _L, _P, _P], _I),
     "ladi_image_out": ([_P, _I, _I, _I, _I, _I, _P, _P], _I),
     "ladi_image_out_u8": ([_P, _I, _I, _I, _I, _I, _P, _P], _I),
+    "ladi_image_save_u8": ([_P, _I, _I, _I, _I, _P, _P], _I),
     "ladi_pose_heatmaps": ([_P, _I, _I, _I, _F, _P, _P], _I),
     "ladi_attention_small": ([_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _L, _L, _L, _L, _F, _I, _P], _I),
     "ladi_attention_small_plan": ([_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _L, _L, _L, _L, _F, _I, _I,

@@ -389,6 +389,16 @@ def image_out_u8(x):
     return out
 
 
+def image_save_u8(x):
+    """NHWC fp32 [n,h,w,>=3] decoder output -> NHWC uint8 [n,h,w,3]: `(x+1)/2` then torchvision save_image's
+    `mul(255).add_(0.5).clamp_(0,255).to(uint8)`, each step rounded in fp32 as torch does it."""
+    n, h, w, _ = x.shape
+    assert x.dtype == torch.float32 and x.stride(3) == 1 and x.stride(1) == w * x.stride(2) and x.stride(0) == h * x.stride(1)
+    out = torch.empty((n, h, w, 3), dtype=torch.uint8, device=x.device)
+    lib.call("ladi_image_save_u8", _ptr(x), n, h, w, x.stride(2), _ptr(out), _stream())
+    return out
+
+
 def pose_heatmaps(keypoints, h, w, sigma=9.0):
     """src/utils/posemap.py kpoint_to_heatmap for a whole batch: keypoints fp32 [..., 2] (x, y) -> fp32 [..., h, w]."""
     k = keypoints.to(torch.float32).contiguous()
