@@ -339,6 +339,12 @@ LADI_API int ladi_tps_grid(const float* theta, int theta_pitch, const float* inv
  * bilinear, padding_mode='border', align_corners=False); cloth NCHW fp32 [n,c,h,w] -> channels [c_off,c_off+c) of NHWC bf16 out. */
 LADI_API int ladi_warp_grid_sample(const float* low_grid, int gh, int gw, const float* cloth, int n, int c, int h, int w, void* out, int out_pitch,
                           int c_off, void* stream);
+/* fp32 forms of ladi_resize_aa and ladi_warp_grid_sample: the same arithmetic, written unrounded as NCHW fp32 [n, c, oh, ow] / [n, c, h, w]
+ * (the bf16 forms store the round-to-nearest bf16 of exactly these values).  The TPS trainer's validation (src/train_tps.py:43-92) reads
+ * the TPS-only warped cloth and the VGG loss's resized inputs in fp32.  x, low_grid, cloth and out 4-byte aligned. */
+LADI_API int ladi_resize_aa_f32(const float* x, int n, int c, int h, int w, int oh, int ow, float* out, void* stream);
+LADI_API int ladi_warp_grid_sample_f32(const float* low_grid, int gh, int gw, const float* cloth, int n, int c, int h, int w, float* out,
+                                       void* stream);
 /* nn.MaxPool2d(2) / nn.Upsample(scale_factor=2, bilinear, align_corners=True) on NHWC bf16 (unet_parts.py:31-34,47).  Dense, c a
  * multiple of 8; x and out 16-byte aligned.  The max pool returns NaN for a window holding a NaN, as nn.MaxPool2d does. */
 LADI_API int ladi_maxpool2_nhwc(const void* x, int n, int h, int w, int c, void* out, void* stream);
@@ -406,6 +412,14 @@ LADI_API int ladi_pool2d_f32(const float* x, int n, int h, int w, int c, int x_p
                              int c_off, void* stream);
 LADI_API int ladi_lpips_layer_f32(const float* fa, const float* fb, int n, int h, int w, int c, int pitch, const float* lin, float* acc,
                                   void* stream);
+/* nn.L1Loss (mean) of two fp32 row-pitched tensors, accumulated on the device: *acc += weight * sum|a - b| / (rows * cols) over
+ * a[r * a_pitch + j], b[r * b_pitch + j], j < cols (the columns past `cols` are never read).  The VGG loss's taps (GEMM output rows) and
+ * NCHW images (rows = n*c*h, cols = w).  Two launches: per-block partial sums into ws (fp32, LADI_L1_MEAN_WS floats), then one block that
+ * sums them in a fixed tree; the grid depends on the shape only, so two runs give the same bits.  Operands 4-byte aligned (16-byte
+ * alignment with cols and pitches multiples of 4 takes the float4 path). */
+#define LADI_L1_MEAN_WS 1024
+LADI_API int ladi_l1_mean_f32(const float* a, int a_pitch, const float* b, int b_pitch, long long rows, int cols, float weight, float* ws,
+                              float* acc, void* stream);
 
 /* ================================================================================================================================
  * Module-level ABI (SURVEY.md section 8(b)): an opaque per-device engine handle + one entry point per module of the try-on path.

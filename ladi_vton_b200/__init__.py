@@ -13,4 +13,5 @@ from .pipeline import StableDiffusionInpaintPipeline, StableDiffusionPipelineOut
 from .scheduler import DDIMScheduler  # noqa: F401
 from .unet import UNet2DConditionModel, unet_param_shapes  # noqa: F401
 from .vae import EMASC, AutoencoderKL, vae_param_shapes  # noqa: F401
+from .vgg import VGG19, VGGLoss  # noqa: F401
 from .warp import ConvNet_TPS, UNetVanilla, generate_warped_cloth  # noqa: F401

@@ -297,6 +297,55 @@ __global__ void __launch_bounds__(256) resize_tf1_kernel(const float* __restrict
   }
 }
 
+// Mean absolute difference of two fp32 row-pitched tensors (nn.L1Loss of the TPS trainer's validation and of its VGG loss):
+// pass 1, block k sums |a - b| over the V-wide column groups k*256 + t, k*256 + t + gridDim*256, ... in thread order, then a fixed tree
+// over its 256 threads -> partial[k]; pass 2, one block sums the partials in the same fixed tree and adds weight * (sum / count) to
+// *acc.  The grid depends on the shape only, so two runs on any device give the same bits.  Pitch padding is never read.
+constexpr int L1_THREADS = 256;
+__device__ __forceinline__ float block_sum_fixed(float v, float* red) {
+  const int t = threadIdx.x;
+  red[t] = v;
+  __syncthreads();
+  for (int o = L1_THREADS / 2; o > 0; o >>= 1) {
+    if (t < o) red[t] += red[t + o];
+    __syncthreads();
+  }
+  return red[0];
+}
+template <int V>
+__global__ void __launch_bounds__(L1_THREADS) l1_partial_kernel(const float* __restrict__ a, long long a_pitch, const float* __restrict__ b,
+                                                                long long b_pitch, int groups_per_row, long long groups,
+                                                                float* __restrict__ partial) {
+  ptx::pdl_wait();
+  __shared__ float red[L1_THREADS];
+  float s = 0.f;
+  for (long long i = (long long)blockIdx.x * L1_THREADS + threadIdx.x; i < groups; i += (long long)gridDim.x * L1_THREADS) {
+    const long long r = i / groups_per_row;
+    const int col = (int)(i - r * groups_per_row) * V;
+    if constexpr (V == 4) {
+      const float4 x = __ldg(reinterpret_cast<const float4*>(a + r * a_pitch + col));
+      const float4 y = __ldg(reinterpret_cast<const float4*>(b + r * b_pitch + col));
+      s += fabsf(x.x - y.x);
+      s += fabsf(x.y - y.y);
+      s += fabsf(x.z - y.z);
+      s += fabsf(x.w - y.w);
+    } else {
+      s += fabsf(__ldg(a + r * a_pitch + col) - __ldg(b + r * b_pitch + col));
+    }
+  }
+  const float t = block_sum_fixed(s, red);
+  if (threadIdx.x == 0) partial[blockIdx.x] = t;
+}
+__global__ void __launch_bounds__(L1_THREADS) l1_final_kernel(const float* __restrict__ partial, int blocks, double count, float weight,
+                                                              float* __restrict__ acc) {
+  ptx::pdl_wait();
+  __shared__ float red[L1_THREADS];
+  float s = 0.f;
+  for (int i = threadIdx.x; i < blocks; i += L1_THREADS) s += partial[i];
+  const float t = block_sum_fixed(s, red);
+  if (threadIdx.x == 0) *acc += weight * (float)((double)t / count);
+}
+
 }  // namespace
 
 static bool aligned_to(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
@@ -450,5 +499,24 @@ extern "C" int ladi_resize_tf1_u8(const float* x, int n, int c, int h, int w, in
   LADI_CHECK(aligned_to(x, 4), "resize_tf1: x %p must be 4-byte aligned", x);
   LADI_CHECK(aligned_to(out, 4), "resize_tf1: out %p must be 4-byte aligned", out);
   LADI_CUDA(ladi_launch(resize_tf1_kernel, dim3(grid_for((long long)n * c * oh * ow)), dim3(256), 0, STREAM, x, h, w, oh, ow, (long long)n * c, out));
+  return LADI_OK;
+}
+
+extern "C" int ladi_l1_mean_f32(const float* a, int a_pitch, const float* b, int b_pitch, long long rows, int cols, float weight, float* ws,
+                                float* acc, void* stream) {
+  LADI_CHECK(a && b && ws && acc && rows > 0 && cols > 0 && a_pitch >= cols && b_pitch >= cols, "l1_mean_f32: bad extent");
+  LADI_CHECK(aligned_to(a, 4) && aligned_to(b, 4) && aligned_to(ws, 4) && aligned_to(acc, 4), "l1_mean_f32: operands must be 4-byte aligned");
+  const bool vec = cols % 4 == 0 && a_pitch % 4 == 0 && b_pitch % 4 == 0 && aligned_to(a, 16) && aligned_to(b, 16);
+  const int v = vec ? 4 : 1;
+  const long long groups = rows * (cols / v);
+  const long long want = (groups + (long long)L1_THREADS * 4 - 1) / ((long long)L1_THREADS * 4);  // ~4 groups per thread
+  const int blocks = (int)(want < 1 ? 1 : (want > LADI_L1_MEAN_WS ? LADI_L1_MEAN_WS : want));
+  if (vec)
+    LADI_CUDA(ladi_launch(l1_partial_kernel<4>, dim3(blocks), dim3(L1_THREADS), 0, STREAM, a, (long long)a_pitch, b, (long long)b_pitch, cols / 4,
+                          groups, ws));
+  else
+    LADI_CUDA(ladi_launch(l1_partial_kernel<1>, dim3(blocks), dim3(L1_THREADS), 0, STREAM, a, (long long)a_pitch, b, (long long)b_pitch, cols,
+                          groups, ws));
+  LADI_CUDA(ladi_launch(l1_final_kernel, dim3(1), dim3(L1_THREADS), 0, STREAM, (const float*)ws, blocks, (double)rows * cols, weight, acc));
   return LADI_OK;
 }

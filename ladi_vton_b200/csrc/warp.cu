@@ -68,9 +68,27 @@ __global__ void __launch_bounds__(256) clip_preprocess_kernel(const float* __res
   }
 }
 
-// x NCHW fp32 [n,c,h,w] -> out NHWC bf16 [n,oh,ow,pitch] channels [c_off, c_off+c)   (torchvision resize(..., BILINEAR, antialias=True))
+// Where the resampling kernels write output pixel `px` (flat over n*oh*ow) of channel ch: NHWC bf16 channels [c_off, c_off+c) of a
+// pitched tensor (the TPS / refinement inputs), or NCHW fp32 [n, c, oh, ow] (the TPS trainer's validation, which reads them unrounded).
+template <typename T> struct ResampleOut;
+template <> struct ResampleOut<bf16> {
+  bf16* p;
+  int pitch, c_off;
+  __device__ __forceinline__ void put(long long px, int, int ch, int, long long, float v) const {
+    p[(size_t)px * pitch + c_off + ch] = __float2bfloat16(v);
+  }
+};
+template <> struct ResampleOut<float> {
+  float* p;
+  __device__ __forceinline__ void put(long long px, int b, int ch, int c, long long hw, float v) const {
+    p[((size_t)b * c + ch) * hw + (px - (long long)b * hw)] = v;
+  }
+};
+
+// x NCHW fp32 [n,c,h,w] -> out (ResampleOut) [n,oh,ow]   (torchvision resize(..., BILINEAR, antialias=True))
+template <typename T>
 __global__ void __launch_bounds__(256) resize_aa_kernel(const float* __restrict__ x, int n, int c, int h, int w, int oh, int ow,
-                                                        bf16* __restrict__ out, int out_pitch, int c_off) {
+                                                        const ResampleOut<T> out) {
   ptx::pdl_wait();
   const long long total = (long long)n * oh * ow;
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
@@ -87,7 +105,7 @@ __global__ void __launch_bounds__(256) resize_aa_kernel(const float* __restrict_
         for (int k = 0; k < tx.count; ++k) r = fmaf(tx.w[k], __ldg(row + k), r);
         acc = fmaf(ty.w[a], r, acc);
       }
-      out[(size_t)i * out_pitch + c_off + ch] = __float2bfloat16(acc);
+      out.put(i, b, ch, c, (long long)oh * ow, acc);
     }
   }
 }
@@ -223,9 +241,10 @@ __global__ void __launch_bounds__(256) tps_grid_kernel(const float* __restrict__
 
 // src/inference.py:252-257: highres_grid = resize(low_grid, (H, W), BILINEAR, antialias=True) ; warped = grid_sample(cloth, highres_grid,
 // mode bilinear, padding_mode 'border', align_corners False).  low_grid [n, gh, gw, 2] fp32, cloth NCHW fp32 [n, c, H, W] (sampled in
-// place at its own resolution), out NHWC bf16 [n, H, W, pitch] channels [c_off, c_off + c).
+// place at its own resolution), out (ResampleOut) [n, H, W].
+template <typename T>
 __global__ void __launch_bounds__(256) warp_sample_kernel(const float* __restrict__ low_grid, int gh, int gw, const float* __restrict__ cloth, int n,
-                                                          int c, int H, int W, bf16* __restrict__ out, int out_pitch, int c_off) {
+                                                          int c, int H, int W, const ResampleOut<T> out) {
   ptx::pdl_wait();
   const long long total = (long long)n * H * W;
   for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
@@ -258,7 +277,7 @@ __global__ void __launch_bounds__(256) warp_sample_kernel(const float* __restric
       if (okx) v = fmaf(wy0 * wx1, __ldg(src + (size_t)y0 * W + x1), v);
       if (oky) v = fmaf(wy1 * wx0, __ldg(src + (size_t)y1 * W + x0), v);
       if (okx && oky) v = fmaf(wy1 * wx1, __ldg(src + (size_t)y1 * W + x1), v);
-      out[(size_t)i * out_pitch + c_off + ch] = __float2bfloat16(v);
+      out.put(i, b, ch, c, (long long)H * W, v);
     }
   }
 }
@@ -361,8 +380,16 @@ extern "C" int ladi_resize_aa(const float* x, int n, int c, int h, int w, int oh
   LADI_CHECK(x && out && n > 0 && c > 0 && h > 0 && w > 0 && oh > 0 && ow > 0, "resize_aa: bad extent");
   LADI_CHECK(out_pitch >= c_off + c, "resize_aa: channel window outside the output pitch");
   LADI_CHECK((float)h / oh <= 5.f && (float)w / ow <= 5.f, "resize_aa: down-scale factors above 5 are not supported");
-  LADI_CUDA(ladi_launch(resize_aa_kernel, dim3(grid_for((long long)n * oh * ow)), dim3(256), 0, STREAM, x, n, c, h, w, oh, ow, (bf16*)out,
-                        out_pitch, c_off));
+  LADI_CUDA(ladi_launch(resize_aa_kernel<bf16>, dim3(grid_for((long long)n * oh * ow)), dim3(256), 0, STREAM, x, n, c, h, w, oh, ow,
+                        ResampleOut<bf16>{(bf16*)out, out_pitch, c_off}));
+  return LADI_OK;
+}
+
+extern "C" int ladi_resize_aa_f32(const float* x, int n, int c, int h, int w, int oh, int ow, float* out, void* stream) {
+  LADI_CHECK(x && out && n > 0 && c > 0 && h > 0 && w > 0 && oh > 0 && ow > 0, "resize_aa_f32: bad extent");
+  LADI_CHECK((float)h / oh <= 5.f && (float)w / ow <= 5.f, "resize_aa_f32: down-scale factors above 5 are not supported");
+  LADI_CUDA(ladi_launch(resize_aa_kernel<float>, dim3(grid_for((long long)n * oh * ow)), dim3(256), 0, STREAM, x, n, c, h, w, oh, ow,
+                        ResampleOut<float>{out}));
   return LADI_OK;
 }
 
@@ -416,8 +443,17 @@ extern "C" int ladi_warp_grid_sample(const float* low_grid, int gh, int gw, cons
   LADI_CHECK(low_grid && cloth && out && n > 0 && c > 0 && gh > 0 && gw > 0 && h > 0 && w > 0, "warp_grid_sample: bad extent");
   LADI_CHECK(out_pitch >= c_off + c, "warp_grid_sample: channel window outside the output pitch");
   LADI_CHECK((float)gh / h <= 5.f && (float)gw / w <= 5.f, "warp_grid_sample: grid down-scale above 5 not supported");
-  LADI_CUDA(ladi_launch(warp_sample_kernel, dim3(grid_for((long long)n * h * w)), dim3(256), 0, STREAM, low_grid, gh, gw, cloth, n, c, h, w,
-                        (bf16*)out, out_pitch, c_off));
+  LADI_CUDA(ladi_launch(warp_sample_kernel<bf16>, dim3(grid_for((long long)n * h * w)), dim3(256), 0, STREAM, low_grid, gh, gw, cloth, n, c, h,
+                        w, ResampleOut<bf16>{(bf16*)out, out_pitch, c_off}));
+  return LADI_OK;
+}
+
+extern "C" int ladi_warp_grid_sample_f32(const float* low_grid, int gh, int gw, const float* cloth, int n, int c, int h, int w, float* out,
+                                         void* stream) {
+  LADI_CHECK(low_grid && cloth && out && n > 0 && c > 0 && gh > 0 && gw > 0 && h > 0 && w > 0, "warp_grid_sample_f32: bad extent");
+  LADI_CHECK((float)gh / h <= 5.f && (float)gw / w <= 5.f, "warp_grid_sample_f32: grid down-scale above 5 not supported");
+  LADI_CUDA(ladi_launch(warp_sample_kernel<float>, dim3(grid_for((long long)n * h * w)), dim3(256), 0, STREAM, low_grid, gh, gw, cloth, n, c, h,
+                        w, ResampleOut<float>{out}));
   return LADI_OK;
 }
 

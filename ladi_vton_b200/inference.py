@@ -90,7 +90,9 @@ class SyntheticTryOnDataset(torch.utils.data.Dataset):
     """N samples with the keys, shapes and value ranges the reference datasets return for `outputlist` (src/dataset/vitonhd.py:109-375):
     image / cloth [3,H,W] in [-1,1], im_mask [3,H,W] (the agnostic person image), pose_map [18,H,W] Gaussian heat-maps,
     inpaint_mask [1,H,W] binary, category str, im_name '<index>.jpg'; for src/eval.py also warped_cloth [3,H,W] in [-1,1], captions
-    (a noun-chunk string) and clip_cloth_features (fp16 [257, clip_dim], the cache of src/utils/compute_cloth_clip_features.py)."""
+    (a noun-chunk string) and clip_cloth_features (fp16 [257, clip_dim], the cache of src/utils/compute_cloth_clip_features.py); for
+    src/train_tps.py also c_name (the cloth's file name), im_cloth [3,H,W] (the person image inside the mask, -1 outside: the garment
+    cut from the person) and dense_uv [2,H,W] in [-1,1] (Dress Code's dense UV map, smooth here)."""
 
     def __init__(self, n, size=(512, 384), categories=('upper_body',), seed=1234, outputlist=None, clip_dim=1280):
         from . import synthetic as S
@@ -111,7 +113,9 @@ class SyntheticTryOnDataset(torch.utils.data.Dataset):
         get = dict(image=lambda: self.a["image"][i], cloth=lambda: self.w["cloth"][i], im_mask=lambda: self.a["image"][i] * (mask < 0.5),
                    pose_map=lambda: self.a["pose_map"][i], inpaint_mask=lambda: mask, category=lambda: cat, im_name=lambda: f"{i:05d}_00.jpg",
                    warped_cloth=lambda: self.a["warped_cloth"][i], captions=lambda: f"{CATEGORY_TEXT[cat].split(' ', 1)[1]}, sample {i}",
-                   clip_cloth_features=lambda: self.clip[i])
+                   clip_cloth_features=lambda: self.clip[i], c_name=lambda: f"{i:05d}_00.jpg",
+                   im_cloth=lambda: torch.where(mask >= 0.5, self.a["image"][i], torch.full_like(self.a["image"][i], -1.0)),
+                   dense_uv=lambda: self.w["pose_map"][i][:2] * 2 - 1)
         return {k: get[k]() for k in self.outputlist}
 
 

@@ -123,6 +123,8 @@ SIGNATURES = {
     "ladi_feature_correlation": ([_P, _P, _I, _I, _I, _I, _P, _I, _P], _I),
     "ladi_tps_grid": ([_P, _I, _P, _P, _I, _I, _I, _P, _P, _P], _I),
     "ladi_warp_grid_sample": ([_P, _I, _I, _P, _I, _I, _I, _I, _P, _I, _I, _P], _I),
+    "ladi_resize_aa_f32": ([_P, _I, _I, _I, _I, _I, _I, _P, _P], _I),
+    "ladi_warp_grid_sample_f32": ([_P, _I, _I, _P, _I, _I, _I, _I, _P, _P], _I),
     "ladi_maxpool2_nhwc": ([_P, _I, _I, _I, _I, _P, _P], _I),
     "ladi_upsample2x_bilinear_ac": ([_P, _I, _I, _I, _I, _P, _P], _I),
     "ladi_nhwc_f32_to_nchw_clamp": ([_P, _I, _I, _I, _I, _I, _F, _F, _P, _P], _I),
@@ -137,6 +139,7 @@ SIGNATURES = {
     "ladi_im2col_f32": ([_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _I, _P], _I),
     "ladi_pool2d_f32": ([_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _I, _I, _P], _I),
     "ladi_lpips_layer_f32": ([_P, _P, _I, _I, _I, _I, _I, _P, _P, _P], _I),
+    "ladi_l1_mean_f32": ([_P, _I, _P, _I, _L, _I, _F, _P, _P, _P], _I),
     # ---- module-level ABI (csrc/engine.cu)
     "ladi_engine_create": ([C.POINTER(EngineConfig), C.POINTER(Weight), _I, _PP], _I),
     "ladi_engine_destroy": ([_P], _I),

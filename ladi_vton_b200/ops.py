@@ -481,6 +481,17 @@ def resize_aa(x, oh, ow, out=None, c_off=0):
     return out
 
 
+def resize_aa_f32(x, oh, ow, out=None):
+    """resize_aa's arithmetic, unrounded: NCHW fp32 -> NCHW fp32 [n, c, oh, ow] (into `out` when given)."""
+    n, c, h, w = x.shape
+    assert x.dtype == torch.float32 and x.is_contiguous()
+    if out is None:
+        out = torch.empty((n, c, oh, ow), dtype=torch.float32, device=x.device)
+    assert out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (n, c, oh, ow)
+    _call("ladi_resize_aa_f32", 0.0, _ptr(x), n, c, h, w, oh, ow, _ptr(out), _stream())
+    return out
+
+
 def clip_preprocess(x, oh, ow, mean, std, quantise=False):
     """inference.py:265-271: resize((x + 1) / 2, (oh, ow), antialias=True).clamp(0, 1) -> (v - mean) / std; NCHW fp32 in and out."""
     n, c, h, w = x.shape
@@ -540,6 +551,16 @@ def warp_grid_sample(low_grid, cloth, out, c_off=0):
     assert low_grid.dtype == torch.float32 and low_grid.is_contiguous() and cloth.dtype == torch.float32 and cloth.is_contiguous()
     assert out.dtype == torch.bfloat16 and out.is_contiguous() and out.shape[:3] == (n, H, W)
     _call("ladi_warp_grid_sample", 0.0, _ptr(low_grid), gh, gw, _ptr(cloth), n, c, H, W, _ptr(out), out.shape[3], c_off, _stream())
+    return out
+
+
+def warp_grid_sample_f32(low_grid, cloth):
+    """warp_grid_sample's arithmetic, unrounded: low_grid fp32 [n,gh,gw,2], cloth NCHW fp32 [n,c,H,W] -> warped NCHW fp32 [n,c,H,W]."""
+    n, gh, gw, _ = low_grid.shape
+    _, c, H, W = cloth.shape
+    assert low_grid.dtype == torch.float32 and low_grid.is_contiguous() and cloth.dtype == torch.float32 and cloth.is_contiguous()
+    out = torch.empty((n, c, H, W), dtype=torch.float32, device=cloth.device)
+    _call("ladi_warp_grid_sample_f32", 0.0, _ptr(low_grid), gh, gw, _ptr(cloth), n, c, H, W, _ptr(out), _stream())
     return out
 
 
@@ -639,6 +660,38 @@ def gemm_tf32(a, weight, n_out, out, c_off=0, bias=None, relu=False):
     _call("ladi_gemm_tf32", 2.0 * m * k * n_out, _ptr(a), m, k, a.stride(0), _ptr(weight), n_out, weight.stride(0), _ptr(bias), int(relu),
           _ptr(out), out.stride(0), c_off, _stream(), tag=f"tf32 M={m} N={n_out} K={k}")
     return out
+
+
+L1_MEAN_WS = 1024  # LADI_L1_MEAN_WS
+_L1_WS = {}
+
+
+def _rows(t):
+    """A 2-D fp32 view [rows, cols] with unit column stride, or a contiguous tensor of any rank seen as [numel / last, last]."""
+    if t.dim() != 2:
+        assert t.is_contiguous(), "l1_mean_: a tensor of rank != 2 must be contiguous"
+        t = t.reshape(-1, t.shape[-1])
+    assert t.dtype == torch.float32 and t.stride(1) == 1
+    return t
+
+
+def l1_mean_(a, b, acc, weight=1.0):
+    """acc[0] += weight * mean|a - b| (nn.L1Loss) on the device, in a fixed reduction order.  a, b: fp32 [rows, cols] views with unit column
+    stride (pitches may differ and exceed cols), or contiguous tensors of equal shape; acc: a one-element fp32 device view.  The partial
+    sums go to a workspace cached per device and stream, so calls issued on different streams do not share one."""
+    a2, b2 = _rows(a), _rows(b)
+    assert a2.shape == b2.shape and acc.dtype == torch.float32 and acc.numel() == 1
+    if lib.RECORD is not None:
+        ws = torch.empty(L1_MEAN_WS, dtype=torch.float32)
+    else:  # the partials of one call are consumed by its own second launch: one workspace per (device, stream) keeps streams apart
+        key = (a.device, torch.cuda.current_stream(a.device).cuda_stream)
+        ws = _L1_WS.get(key)
+        if ws is None:
+            ws = _L1_WS[key] = torch.empty(L1_MEAN_WS, dtype=torch.float32, device=a.device)
+    rows, cols = a2.shape
+    _call("ladi_l1_mean_f32", 3.0 * rows * cols, _ptr(a2), a2.stride(0), _ptr(b2), b2.stride(0), rows, cols, float(weight), _ptr(ws), _ptr(acc),
+          _stream(), tag=f"rows={rows} cols={cols}")
+    return acc
 
 
 def ssim(x, y):

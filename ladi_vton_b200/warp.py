@@ -263,24 +263,52 @@ class UNetVanilla(_Module):
         return ops.nhwc_f32_to_nchw_clamp(y, self.n_classes, -3.0e38, 3.0e38)
 
 
-def generate_warped_cloth(tps, refinement, cloth, im_mask, pose_map):
-    """The warping part of the reference's inference loop body (src/inference.py:236-263): cloth [B,3,H,W] in [-1,1], im_mask [B,3,H,W],
-    pose_map [B,18,H,W] -> refined warped cloth NCHW fp32 in [-1,1] (the `warped_cloth` argument of the try-on pipeline)."""
-    dev = tps.device
-    B, cc, H, W = cloth.shape
-    lh, lw = tps.height, tps.width  # (256, 192): the TPS parameters are predicted at low resolution (:236-247)
-    cloth_d = cloth.to(dev, torch.float32).contiguous()
-    mask_d = im_mask.to(dev, torch.float32).contiguous()
-    pose_d = pose_map.to(dev, torch.float32).contiguous()
+def _low_grid(tps, cloth_d, mask_d, pose_d):
+    """inference.py:236-247 (= train_tps.py:53-68): the three antialiased resizes to the TPS resolution and the TPS forward ->
+    low-resolution sampling grid fp32 [B, lh, lw, 2]."""
+    B, cc = cloth_d.shape[:2]
+    lh, lw = tps.height, tps.width  # (256, 192): the TPS parameters are predicted at low resolution
     cm, cp = mask_d.shape[1], pose_d.shape[1]
     low_cloth = ops.resize_aa(cloth_d, lh, lw)
-    agnostic = torch.zeros((B, lh, lw, (cm + cp + 7) // 8 * 8), dtype=torch.bfloat16, device=dev)
+    agnostic = torch.zeros((B, lh, lw, (cm + cp + 7) // 8 * 8), dtype=torch.bfloat16, device=cloth_d.device)
     ops.resize_aa(mask_d, lh, lw, out=agnostic, c_off=0)
     ops.resize_aa(pose_d, lh, lw, out=agnostic, c_off=cm)  # torch.cat([low_im_mask, low_pose_map], 1)  (:247)
     low_grid, _ = tps.forward_nhwc(low_cloth, cc, agnostic, cm + cp)
+    return low_grid
+
+
+def _on(dev, *ts):
+    return [t.to(dev, torch.float32).contiguous() for t in ts]
+
+
+def _refine(tps, refinement, cloth, im_mask, pose_map, lo, hi):
+    dev = tps.device
+    cloth_d, mask_d, pose_d = _on(dev, cloth, im_mask, pose_map)
+    B, cc, H, W = cloth_d.shape
+    cm, cp = mask_d.shape[1], pose_d.shape[1]
+    low_grid = _low_grid(tps, cloth_d, mask_d, pose_d)
     x = torch.zeros((B, H, W, (cm + cp + cc + 7) // 8 * 8), dtype=torch.bfloat16, device=dev)
     ops.nchw_to_nhwc(mask_d, x, c_off=0)  # torch.cat([im_mask, pose_map, warped_cloth], 1)  (:260)
     ops.nchw_to_nhwc(pose_d, x, c_off=cm)
     ops.warp_grid_sample(low_grid, cloth_d, x, c_off=cm + cp)  # grid resize (:252-255) + grid_sample (:257)
     y = refinement.forward_nhwc(x)
-    return ops.nhwc_f32_to_nchw_clamp(y, refinement.n_classes, -1.0, 1.0)  # :262
+    return ops.nhwc_f32_to_nchw_clamp(y, refinement.n_classes, lo, hi)
+
+
+def generate_warped_cloth(tps, refinement, cloth, im_mask, pose_map):
+    """The warping part of the reference's inference loop body (src/inference.py:236-263): cloth [B,3,H,W] in [-1,1], im_mask [B,3,H,W],
+    pose_map [B,18,H,W] -> refined warped cloth NCHW fp32 in [-1,1] (the `warped_cloth` argument of the try-on pipeline)."""
+    return _refine(tps, refinement, cloth, im_mask, pose_map, -1.0, 1.0)  # :262
+
+
+def refine_warped_cloth(tps, refinement, cloth, im_mask, pose_map):
+    """generate_warped_cloth without the final clamp: the refinement network's output as the TPS trainer scores it (train_tps.py:77-80;
+    UNetVanilla.__call__ returns it unclamped too)."""
+    return _refine(tps, refinement, cloth, im_mask, pose_map, -3.0e38, 3.0e38)
+
+
+def tps_warped_cloth(tps, cloth, im_mask, pose_map):
+    """The TPS-only warp of the trainer's validation (train_tps.py:53-75, `refinement=None`): the same resizes, TPS and grid sampling as
+    generate_warped_cloth -> the sampled cloth itself, NCHW fp32 [B, 3, H, W], unrounded (`ladi_warp_grid_sample_f32`)."""
+    cloth_d, mask_d, pose_d = _on(tps.device, cloth, im_mask, pose_map)
+    return ops.warp_grid_sample_f32(_low_grid(tps, cloth_d, mask_d, pose_d), cloth_d)
