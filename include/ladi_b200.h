@@ -143,13 +143,31 @@ typedef struct ladi_attn_desc {
   void* trace;               /* unused (NULL) */
   int head_dim;              /* ladi_attention_d512_bf16 only: 0 or 512 (the VAE), or 256 (reduced-width test models) */
 } ladi_attn_desc;
-/* Placement rules of both attention entry points (LADI_ERR_INVALID when broken): q, k, v 16-byte aligned, every pitch a multiple of 8
- * and >= the head columns (heads*64, or head_dim), out 4-byte aligned (it is stored as bf16 pairs) with an even out_batch_stride. */
+/* Placement rules of both attention entry points (LADI_ERR_INVALID when broken): q, k, v 16-byte aligned with batch strides that are
+ * multiples of 8 (TMA: 16-byte global addresses and strides), every pitch a multiple of 8 and >= the head columns (heads*64, or
+ * head_dim), out 4-byte aligned (it is stored as bf16 pairs) with an even out_batch_stride. */
 LADI_API int ladi_attention_bf16(const ladi_attn_desc* d, void* stream);
 /* The same for ONE head of width 512: the VAE mid-block AttentionBlock (src/models/vae.py:81-90,112 encoder; :142-150,187 decoder;
  * N = h*w tokens: 3072 at 512x384, 12288 at 1024x768).  heads must be 1, pitches >= head_dim; `variant` / `trace` ignored.  Flash-style:
  * the N x N score matrix is never written (the reference's baddbmm + softmax + bmm materialises it per sample). */
 LADI_API int ladi_attention_d512_bf16(const ladi_attn_desc* d, void* stream);
+/* The launch ladi_attention_bf16 (wide = 0) or ladi_attention_d512_bf16 (wide != 0) runs for `d` on a device with `sms` SMs (sms <= 0:
+ * the current device's count).  head_dim 64 is attention_d64_kernel: persistent, grid_x = min(n_items, sms) CTAs, where an item is one
+ * (query tile, head, image), numbered query tile fastest, and CTA c runs items c, c + grid_x, ...  (items_min / items_max per CTA).
+ * head_dim 512 / 256 is attention_kernel<D>: one CTA per (query tile, 128-column output slice, image), n_items = grid_x*grid_y*grid_z.
+ * q_tile / kv_tile are the query rows and keys of one tile, stages the K / V ring depth (D = 64: K and V tile pairs; wide: 64-column
+ * chunks), consumers the warpgroups that each own 64 query rows of a tile; idle_consumers_last_q_tile of them have no row in the
+ * last query tile.  The same validation and policy code as the launches; it dereferences no pointer and needs no device. */
+typedef struct ladi_attn_plan {
+  int head_dim;
+  int grid_x, grid_y, grid_z;
+  int q_tile, kv_tile, stages, consumers;
+  int n_q_tiles, n_kv_tiles, n_items;
+  int items_min, items_max;
+  int idle_consumers_last_q_tile;
+  int smem_bytes;
+} ladi_attn_plan;
+LADI_API int ladi_attention_plan(const ladi_attn_desc* d, int wide, int sms, ladi_attn_plan* out);
 
 /* ---- normalisation ---------------------------------------------------------------------------------------------------
  * GroupNorm(+SiLU) over the channel-concat of up to two NHWC sources (diffusers ResnetBlock2D.norm1/norm2,

@@ -498,7 +498,7 @@ int make_map(CUtensorMap* m, const void* ptr, int cols, int tokens, int batch, i
 }
 
 template <int D>
-int launch(const ladi_attn_desc* d, int cols, dim3 grid, cudaStream_t stream) {
+int launch(const ladi_attn_desc* d, const ladi_attn_plan& pl, cudaStream_t stream) {
   using C = AttnCfg<D>;
   static bool attr_set = false;
   if (!attr_set) {
@@ -506,37 +506,89 @@ int launch(const ladi_attn_desc* d, int cols, dim3 grid, cudaStream_t stream) {
     attr_set = true;
   }
   CUtensorMap tq, tk, tv;
-  if (make_map(&tq, d->q, cols, d->nq, d->batch, d->q_pitch, d->q_batch_stride, BQ)) return LADI_ERR_CUDA;
-  if (make_map(&tk, d->k, cols, d->nkv, d->batch, d->k_pitch, d->k_batch_stride, C::BKV)) return LADI_ERR_CUDA;
-  if (make_map(&tv, d->v, cols, d->nkv, d->batch, d->v_pitch, d->v_batch_stride, C::BKV)) return LADI_ERR_CUDA;
+  if (make_map(&tq, d->q, D, d->nq, d->batch, d->q_pitch, d->q_batch_stride, BQ)) return LADI_ERR_CUDA;
+  if (make_map(&tk, d->k, D, d->nkv, d->batch, d->k_pitch, d->k_batch_stride, C::BKV)) return LADI_ERR_CUDA;
+  if (make_map(&tv, d->v, D, d->nkv, d->batch, d->v_pitch, d->v_batch_stride, C::BKV)) return LADI_ERR_CUDA;
   AttnParams p;
-  p.nq = d->nq; p.nkv = d->nkv; p.n_kv_tiles = (d->nkv + C::BKV - 1) / C::BKV;
+  p.nq = d->nq; p.nkv = d->nkv; p.n_kv_tiles = pl.n_kv_tiles;
   p.out = reinterpret_cast<bf16*>(d->out); p.out_pitch = d->out_pitch; p.out_batch_stride = d->out_batch_stride;
   p.scale_log2 = d->scale * 1.4426950408889634f;
-  LADI_CUDA(ladi_launch(attention_kernel<D>, grid, dim3(384), C::SMEM, stream, tq, tk, tv, p));
+  LADI_CUDA(ladi_launch(attention_kernel<D>, dim3(pl.grid_x, pl.grid_y, pl.grid_z), dim3(384), C::SMEM, stream, tq, tk, tv, p));
   return LADI_OK;
 }
 
-// Both kernels store the output as bf16 pairs (4 bytes): out must be 4-byte aligned and every batch's rows start on a pair.
-int check_out_placement(const ladi_attn_desc* d) {
-  LADI_CHECK((reinterpret_cast<uintptr_t>(d->out) & 3) == 0, "out %p must be 4-byte aligned", d->out);
+bool aligned_to(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
+// Everything the two attention launches decide from the descriptor and the SM count alone (no pointer is dereferenced, nothing touches
+// a device): validation, the kernel's tile constants and its grid.  ladi_attention_plan reports it; ladi_attention_bf16 (wide = 0) and
+// ladi_attention_d512_bf16 (wide = 1) launch it.  Q, K and V are read by TMA (16-byte aligned base, strides multiples of 16 bytes); both
+// kernels store the output as bf16 pairs (4 bytes): out must be 4-byte aligned and every batch's rows start on a pair.
+int attn_plan(const ladi_attn_desc* d, int wide, int sms, ladi_attn_plan& pl) {
+  LADI_CHECK(d != nullptr && d->q && d->k && d->v && d->out, "null attention operand");
+  if (wide) {
+    LADI_CHECK(d->batch > 0 && d->heads == 1 && d->nq > 0 && d->nkv > 0, "d512 attention: one head, non-empty extents");
+  } else {
+    LADI_CHECK(d->batch > 0 && d->heads > 0 && d->nq > 0 && d->nkv > 0, "bad attention extent");
+  }
+  LADI_CHECK(d->q_pitch % 8 == 0 && d->k_pitch % 8 == 0 && d->v_pitch % 8 == 0 && d->out_pitch % 8 == 0, "pitches must be multiples of 8");
+  const int D = wide ? (d->head_dim == 0 ? 512 : d->head_dim) : 64;
+  if (wide) {
+    LADI_CHECK(D == 512 || D == 256, "wide attention: head_dim must be 512 (or 256), got %d", D);
+    LADI_CHECK(d->q_pitch >= D && d->k_pitch >= D && d->v_pitch >= D && d->out_pitch >= D, "pitch < head_dim");
+  } else {
+    LADI_CHECK(d->q_pitch >= d->heads * 64 && d->k_pitch >= d->heads * 64 && d->v_pitch >= d->heads * 64 && d->out_pitch >= d->heads * 64,
+               "pitch < heads*64");
+  }
+  LADI_CHECK(aligned_to(d->q, 16), "q %p must be 16-byte aligned (TMA)", d->q);
+  LADI_CHECK(aligned_to(d->k, 16), "k %p must be 16-byte aligned (TMA)", d->k);
+  LADI_CHECK(aligned_to(d->v, 16), "v %p must be 16-byte aligned (TMA)", d->v);
+  LADI_CHECK(d->q_batch_stride % 8 == 0, "q_batch_stride %lld must be a multiple of 8 (TMA)", (long long)d->q_batch_stride);
+  LADI_CHECK(d->k_batch_stride % 8 == 0, "k_batch_stride %lld must be a multiple of 8 (TMA)", (long long)d->k_batch_stride);
+  LADI_CHECK(d->v_batch_stride % 8 == 0, "v_batch_stride %lld must be a multiple of 8 (TMA)", (long long)d->v_batch_stride);
+  LADI_CHECK(aligned_to(d->out, 4), "out %p must be 4-byte aligned", d->out);
   LADI_CHECK(d->out_batch_stride % 2 == 0, "out_batch_stride %lld must be even", (long long)d->out_batch_stride);
+  if (!wide)
+    LADI_CHECK(d->variant == 0 || d->variant == 1 || d->variant == 2 || d->variant == 4 || d->variant == 5 || d->variant == 6 ||
+                   (d->variant == 8 && d->nkv <= 128),
+               "bad attention variant %d", d->variant);
+  pl.head_dim = D;
+  if (wide) {
+    pl.q_tile = BQ; pl.kv_tile = 64; pl.consumers = 2;
+    pl.stages = D == 512 ? AttnCfg<512>::STAGES : AttnCfg<256>::STAGES;
+    pl.smem_bytes = (int)(D == 512 ? AttnCfg<512>::SMEM : AttnCfg<256>::SMEM);
+  } else {
+    pl.q_tile = Attn64::BQ; pl.kv_tile = Attn64::BKV; pl.consumers = Attn64::NWG; pl.stages = Attn64::STAGES;
+    pl.smem_bytes = (int)Attn64::SMEM;
+  }
+  pl.n_q_tiles = (d->nq + pl.q_tile - 1) / pl.q_tile;
+  pl.n_kv_tiles = (d->nkv + pl.kv_tile - 1) / pl.kv_tile;
+  const int last_rows = d->nq - (pl.n_q_tiles - 1) * pl.q_tile;
+  pl.idle_consumers_last_q_tile = pl.consumers - (last_rows + 63) / 64;
+  if (wide) {
+    pl.grid_x = pl.n_q_tiles; pl.grid_y = D / 128; pl.grid_z = d->batch;
+    pl.n_items = pl.grid_x * pl.grid_y * pl.grid_z;
+    pl.items_min = pl.items_max = 1;
+  } else {
+    // persistent: at most one CTA per SM (the kernel's registers and shared memory allow no second one)
+    pl.n_items = pl.n_q_tiles * d->heads * d->batch;
+    pl.grid_x = std::min(pl.n_items, sms); pl.grid_y = pl.grid_z = 1;
+    pl.items_min = pl.n_items / pl.grid_x;
+    pl.items_max = (pl.n_items + pl.grid_x - 1) / pl.grid_x;
+  }
   return LADI_OK;
 }
 
 }  // namespace
 
+extern "C" int ladi_attention_plan(const ladi_attn_desc* d, int wide, int sms, ladi_attn_plan* out) {
+  LADI_CHECK(out != nullptr, "plan output is null");
+  return attn_plan(d, wide, sms > 0 ? sms : ladi_num_sms(), *out);
+}
+
 extern "C" int ladi_attention_bf16(const ladi_attn_desc* d, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  LADI_CHECK(d != nullptr && d->q && d->k && d->v && d->out, "null attention operand");
-  LADI_CHECK(d->batch > 0 && d->heads > 0 && d->nq > 0 && d->nkv > 0, "bad attention extent");
-  LADI_CHECK(d->q_pitch % 8 == 0 && d->k_pitch % 8 == 0 && d->v_pitch % 8 == 0 && d->out_pitch % 8 == 0, "pitches must be multiples of 8");
-  LADI_CHECK(d->q_pitch >= d->heads * 64 && d->k_pitch >= d->heads * 64 && d->v_pitch >= d->heads * 64 && d->out_pitch >= d->heads * 64,
-             "pitch < heads*64");
-  if (const int rc = check_out_placement(d)) return rc;
-  LADI_CHECK(d->variant == 0 || d->variant == 1 || d->variant == 2 || d->variant == 4 || d->variant == 5 || d->variant == 6 ||
-                 (d->variant == 8 && d->nkv <= 128),
-             "bad attention variant %d", d->variant);
+  ladi_attn_plan pl;
+  if (const int rc = attn_plan(d, 0, ladi_num_sms(), pl)) return rc;
   using C = Attn64;
   static bool attr_set = false;
   if (!attr_set) {
@@ -549,27 +601,17 @@ extern "C" int ladi_attention_bf16(const ladi_attn_desc* d, void* stream_) {
   if (make_map(&tk, d->k, cols, d->nkv, d->batch, d->k_pitch, d->k_batch_stride, C::BKV)) return LADI_ERR_CUDA;
   if (make_map(&tv, d->v, cols, d->nkv, d->batch, d->v_pitch, d->v_batch_stride, C::BKV)) return LADI_ERR_CUDA;
   AttnParams p;
-  p.nq = d->nq; p.nkv = d->nkv; p.n_kv_tiles = (d->nkv + C::BKV - 1) / C::BKV;
+  p.nq = d->nq; p.nkv = d->nkv; p.n_kv_tiles = pl.n_kv_tiles;
   p.out = reinterpret_cast<bf16*>(d->out); p.out_pitch = d->out_pitch; p.out_batch_stride = d->out_batch_stride;
   p.scale_log2 = d->scale * 1.4426950408889634f;
-  p.n_q_tiles = (d->nq + C::BQ - 1) / C::BQ; p.heads = d->heads; p.n_items = p.n_q_tiles * d->heads * d->batch;
-  int dev = 0, sms = 0;
-  LADI_CUDA(cudaGetDevice(&dev));
-  LADI_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  // persistent: at most one CTA per SM (the kernel's registers and shared memory allow no second one)
-  LADI_CUDA(ladi_launch(attention_d64_kernel, dim3(std::min(p.n_items, sms)), dim3(C::THREADS), C::SMEM, stream, tq, tk, tv, p));
+  p.n_q_tiles = pl.n_q_tiles; p.heads = d->heads; p.n_items = pl.n_items;
+  LADI_CUDA(ladi_launch(attention_d64_kernel, dim3(pl.grid_x, pl.grid_y, pl.grid_z), dim3(C::THREADS), C::SMEM, stream, tq, tk, tv, p));
   return LADI_OK;
 }
 
 extern "C" int ladi_attention_d512_bf16(const ladi_attn_desc* d, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  LADI_CHECK(d != nullptr && d->q && d->k && d->v && d->out, "null attention operand");
-  LADI_CHECK(d->batch > 0 && d->heads == 1 && d->nq > 0 && d->nkv > 0, "d512 attention: one head, non-empty extents");
-  LADI_CHECK(d->q_pitch % 8 == 0 && d->k_pitch % 8 == 0 && d->v_pitch % 8 == 0 && d->out_pitch % 8 == 0, "pitches must be multiples of 8");
-  const int D5 = d->head_dim == 0 ? 512 : d->head_dim;
-  LADI_CHECK(D5 == 512 || D5 == 256, "wide attention: head_dim must be 512 (or 256), got %d", D5);
-  LADI_CHECK(d->q_pitch >= D5 && d->k_pitch >= D5 && d->v_pitch >= D5 && d->out_pitch >= D5, "pitch < head_dim");
-  if (const int rc = check_out_placement(d)) return rc;
-  const dim3 grid((d->nq + BQ - 1) / BQ, D5 / 128, d->batch);
-  return D5 == 512 ? launch<512>(d, D5, grid, stream) : launch<256>(d, D5, grid, stream);
+  ladi_attn_plan pl;
+  if (const int rc = attn_plan(d, 1, ladi_num_sms(), pl)) return rc;
+  return pl.head_dim == 512 ? launch<512>(d, pl, stream) : launch<256>(d, pl, stream);
 }

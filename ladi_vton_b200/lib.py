@@ -49,6 +49,11 @@ class SmallAttnPlan(C.Structure):  # ladi_sa_plan (ladi_attention_small_plan, la
     _fields_ = [(f, C.c_int) for f in ("chunks", "rows_per_block", "smem_bytes", "smem_optin")]
 
 
+class AttnPlan(C.Structure):  # ladi_attn_plan (ladi_attention_plan): the launch ladi_attention_bf16 / ladi_attention_d512_bf16 run
+    _fields_ = [(f, C.c_int) for f in ("head_dim", "grid_x", "grid_y", "grid_z", "q_tile", "kv_tile", "stages", "consumers", "n_q_tiles",
+                                        "n_kv_tiles", "n_items", "items_min", "items_max", "idle_consumers_last_q_tile", "smem_bytes")]
+
+
 class AttnDesc(C.Structure):
     _fields_ = [
         ("batch", C.c_int), ("heads", C.c_int), ("nq", C.c_int), ("nkv", C.c_int),
@@ -87,6 +92,7 @@ SIGNATURES = {
     "ladi_conv2d_plan": ([C.POINTER(ConvDesc), _I, C.POINTER(ConvPlan)], _I),
     "ladi_attention_bf16": ([C.POINTER(AttnDesc), _P], _I),
     "ladi_attention_d512_bf16": ([C.POINTER(AttnDesc), _P], _I),
+    "ladi_attention_plan": ([C.POINTER(AttnDesc), _I, _I, C.POINTER(AttnPlan)], _I),
     "ladi_groupnorm_chunks": ([_I], _I),
     "ladi_groupnorm_stats": ([_P, _I, _I, _P, _I, _I, _I, _I, _I, _P, _P], _I),
     "ladi_groupnorm_apply": ([_P, _I, _I, _P, _I, _I, _I, _I, _I, _P, _P, _P, _F, _I, _P, _I, _P, _I, _P], _I),

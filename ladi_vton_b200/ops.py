@@ -181,19 +181,8 @@ def gemm_plan(a, weight, n_out, sms=0, **kw):
 
 def attention(q, k, v, heads, scale, out=None, variant=0, trace=None):
     """q [B, Nq, >=heads*64] , k/v [B, Nkv, >=heads*64] (row-strided views of fused projections are fine) -> [B, Nq, heads*64]."""
-    B, nq = q.shape[0], q.shape[1]
-    nkv = k.shape[1]
-    for t in (q, k, v):
-        assert t.dtype == torch.bfloat16 and t.stride(2) == 1
-    if out is None:
-        out = torch.empty((B, nq, heads * 64), dtype=torch.bfloat16, device=q.device)
-    d = AttnDesc()
-    d.batch, d.heads, d.nq, d.nkv = B, heads, nq, nkv
-    d.q, d.q_pitch, d.q_batch_stride = q.data_ptr(), q.stride(1), q.stride(0)
-    d.k, d.k_pitch, d.k_batch_stride = k.data_ptr(), k.stride(1), k.stride(0)
-    d.v, d.v_pitch, d.v_batch_stride = v.data_ptr(), v.stride(1), v.stride(0)
-    d.out, d.out_pitch, d.out_batch_stride = out.data_ptr(), out.stride(1), out.stride(0)
-    d.scale = scale
+    B, nq, nkv = q.shape[0], q.shape[1], k.shape[1]
+    d, out = _attention_desc(q, k, v, heads, heads * 64, scale, out)
     d.variant = variant
     d.trace = trace.data_ptr() if trace is not None else 0
     _call("ladi_attention_bf16", 4.0 * B * heads * nq * nkv * 64, C.byref(d), _stream(), tag=f"B={B} heads={heads} nq={nq} nkv={nkv}")
@@ -206,18 +195,42 @@ def attention_d512(q, k, v, scale, out=None):
     B, nq, nkv, D = q.shape[0], q.shape[1], k.shape[1], q.shape[2]
     assert D in (256, 512), "the wide single-head attention kernel is built for head widths 512 and 256"
     for t in (q, k, v):
-        assert t.dtype == torch.bfloat16 and t.stride(2) == 1 and t.shape[2] == D
+        assert t.shape[2] == D
+    d, out = _attention_desc(q, k, v, 1, D, scale, out)
+    d.head_dim = D
+    _call("ladi_attention_d512_bf16", 4.0 * B * nq * nkv * D, C.byref(d), _stream(), tag=f"B={B} d{D} nq={nq} nkv={nkv}")
+    return out
+
+
+def attention_plan(q, k, v, heads, scale, wide=False, sms=0):
+    """The launch (lib.AttnPlan: grid, tiles, work items per CTA, idle consumer warpgroups, shared memory) attention(q, k, v, heads,
+    scale) -- or, with wide=True, attention_d512(q, k, v, scale) (heads 1, head width q.shape[2]) -- runs on a device with `sms` SMs (0:
+    this one's); launches nothing.  Invalid -> RuntimeError."""
+    D = q.shape[2] if wide else 64
+    d, _ = _attention_desc(q, k, v, heads, heads * D, scale, None)
+    d.head_dim = D if wide else 0
+    plan = lib.AttnPlan()
+    L = lib.load()
+    if L.ladi_attention_plan(C.byref(d), 1 if wide else 0, sms, C.byref(plan)) != 0:
+        raise RuntimeError(f"ladi_attention_plan failed: {L.ladi_last_error().decode()}")
+    return plan
+
+
+def _attention_desc(q, k, v, heads, width, scale, out):
+    """-> (the lib.AttnDesc of q, k, v and out, the output tensor [B, Nq, width] it writes)."""
+    B, nq = q.shape[0], q.shape[1]
+    for t in (q, k, v):
+        assert t.dtype == torch.bfloat16 and t.stride(2) == 1
     if out is None:
-        out = torch.empty((B, nq, D), dtype=torch.bfloat16, device=q.device)
+        out = torch.empty((B, nq, width), dtype=torch.bfloat16, device=q.device)
     d = AttnDesc()
-    d.batch, d.heads, d.nq, d.nkv = B, 1, nq, nkv
+    d.batch, d.heads, d.nq, d.nkv = B, heads, nq, k.shape[1]
     d.q, d.q_pitch, d.q_batch_stride = q.data_ptr(), q.stride(1), q.stride(0)
     d.k, d.k_pitch, d.k_batch_stride = k.data_ptr(), k.stride(1), k.stride(0)
     d.v, d.v_pitch, d.v_batch_stride = v.data_ptr(), v.stride(1), v.stride(0)
     d.out, d.out_pitch, d.out_batch_stride = out.data_ptr(), out.stride(1), out.stride(0)
-    d.scale, d.head_dim = scale, D
-    _call("ladi_attention_d512_bf16", 4.0 * B * nq * nkv * D, C.byref(d), _stream(), tag=f"B={B} d{D} nq={nq} nkv={nkv}")
-    return out
+    d.scale = scale
+    return d, out
 
 
 class GroupNormWS:

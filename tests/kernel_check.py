@@ -16,6 +16,8 @@ The error bound is per element and is built from the error sources the kernels h
   ACT_GAIN = 1.13   sup |act'| of SiLU (1.10) and GELU (1.13): how much an accumulation error grows through the activation;
   U_P      = 2^-7   attention: P is rounded to bf16 (2^-8) before P.V, doubled; the error it causes is at most U_P * sum p|v| / l;
   E_EXP    = 2^-16  attention: ex2.approx (2^-22 relative) plus the fp32 rounding of the exponent argument (|x| 2^-24, |x| < 2^6);
+                    its domain is |x| < 2^6 for x = scale log2(e) q.k, which every attention test input keeps (EXP2_DOMAIN; attn_inputs
+                    asserts it for the wgmma kernels' score distributions);
   ROUND1   = 2^-8   one round-to-nearest to bf16 (8-bit significand).
 So  conv/GEMM:  |y - r| <= U * |r| + gain * C_ACC * sqrt(K) * 2^-24 * m + eps_act,  m = |A| (*) |W| + |bias| + |residual| in float64;
     attention:  |y - r| <= U * |r| + (U_P + C_ACC * sqrt(nkv) * 2^-24 + E_EXP) * sum p|v| / l   (from the float64 softmax);
@@ -838,6 +840,133 @@ def attn_ref(q, k, v, heads, D, scale):
         sv[:, i:i + ch] = (p @ vh.abs()) / l
         del p
     return o.transpose(0, 1).reshape(nq, heads * D), sv.transpose(0, 1).reshape(nq, heads * D)
+
+
+# ================================================================================================================ flash attention: inputs, emulation
+# Score distributions of the wgmma attention tests, in exp2 units x = scale log2(e) q.k (the kernels' softmax argument before the
+# running maximum is subtracted).  Each stays inside the domain E_EXP is stated for, |x| < EXP2_DOMAIN (attn_inputs asserts it):
+#   randn  q, k ~ N(0, 2), v ~ N(0, 1): the census's inputs; |x| reaches about 17;
+#   late   the key scores rise by a step (<= 6) on every key tile, from -48 to at most +48: the maximum moves up on every tile, so l and O
+#          are rescaled on every tile;
+#   early  one key of tile 0 at x = 4, every other key about 40 lower: later tiles add P <= 2^-40 and alpha is exactly 1 after tile 0;
+#   tail   the last key scores exactly 0 (a zero key), every other key about -6: the row maximum sits in the ragged last tile beside the
+#          masked lanes, whose zero-filled keys would also score 0;
+#   flat   q = 0, so every score is exactly 0: the output is the mean of V over the valid keys (v = 1 + N(0, 1/4), so the mean is far
+#          from 0 and a counted padded key moves it by 1 / (nkv + 1));
+#   level  scores ~ N(0, 1.5^2) around a constant offset per (image, head), the offsets spread over [-48, 48] and interleaved so that
+#          consecutive (image, head) pairs, and the consecutive work items of a persistent CTA, run at very different levels.
+# The structured forms (late, early, tail, level) build q = u + 0.1 n and k = t / (scale log2(e) D) u + sigma n along one sign vector u
+# per head (u.u = D), so that x = t plus a few tenths of noise for a target t per key.
+ATTN_DISTS = ("randn", "late", "early", "tail", "flat", "level")
+EXP2_DOMAIN = 2.0 ** 6
+L2E = 1.4426950408889634
+
+
+def _levels(n):
+    """n offsets spread over [-48, 48], in the order lowest, highest, second lowest, second highest, ..."""
+    lv = torch.linspace(-48.0, 48.0, n) if n > 1 else torch.tensor([-48.0])
+    order = [i // 2 if i % 2 == 0 else n - 1 - i // 2 for i in range(n)]
+    return lv[order]
+
+
+def score_range(q, k, heads, D, scale):
+    """-> max |scale log2(e) q.k| over every head, query and key of q [nq, heads*D], k [nkv, heads*D] (float64, chunked)."""
+    nq, nkv = q.shape[0], k.shape[0]
+    ch = max(1, (1 << 24) // nkv)
+    worst = 0.0
+    for h in range(heads):
+        qh, kh = q[:, h * D:(h + 1) * D].double(), k[:, h * D:(h + 1) * D].double()
+        for i in range(0, nq, ch):
+            worst = max(worst, float((qh[i:i + ch] @ kh.t()).abs().max()) * scale * L2E)
+    return worst
+
+
+def attn_inputs(dist, gen, B, heads, nq, nkv, D, scale, tile):
+    """bf16 q [B, nq, heads*D], k / v [B, nkv, heads*D] with the score distribution `dist` (above) for a kernel with `tile`-key tiles,
+    drawn from `gen` on its device."""
+    assert dist in ATTN_DISTS, dist
+    dev = gen.device
+    W = heads * D
+    rn = lambda *s: torch.randn(s, generator=gen, device=dev)  # noqa: E731
+    if dist == "randn":
+        q, k, v = (rn(B, nq, W) * 2 ** 0.5).bfloat16(), (rn(B, nkv, W) * 2 ** 0.5).bfloat16(), rn(B, nkv, W).bfloat16()
+    elif dist == "flat":
+        q, k, v = torch.zeros((B, nq, W), device=dev).bfloat16(), (rn(B, nkv, W) * 2 ** 0.5).bfloat16(), (1.0 + 0.5 * rn(B, nkv, W)).bfloat16()
+    else:
+        c = scale * L2E
+        u = torch.sign(rn(1, heads, 1, D))  # [1, heads, 1, D]
+        j = torch.arange(nkv, device=dev, dtype=torch.float32)
+        sigma = 0.5
+        if dist == "late":
+            nt = -(-nkv // tile)
+            t = (-48.0 + min(6.0, 96.0 / max(1, nt - 1)) * torch.div(j, tile, rounding_mode="floor")).expand(B, heads, nkv)
+        elif dist == "early":
+            t = torch.full((B, heads, nkv), -40.0, device=dev)
+            t[..., 37 % min(nkv, tile)] = 4.0
+        elif dist == "tail":
+            t = torch.full((B, heads, nkv), -6.0, device=dev)
+        else:  # level
+            t = _levels(B * heads).to(dev).view(B, heads, 1).expand(B, heads, nkv)
+            sigma = 1.0
+        q = u + 0.1 * rn(B, heads, nq, D)
+        k = (t[..., None] / (c * D)) * u + sigma * rn(B, heads, nkv, D)
+        if dist == "early":
+            k[:, :, 37 % min(nkv, tile)] = (4.0 / (c * D)) * u[:, :, 0]  # the maximum without noise: x = 4 (1 + 0.1 u.n / D)
+        elif dist == "tail":
+            k[:, :, nkv - 1] = 0.0
+        q, k = (t_.permute(0, 2, 1, 3).reshape(B, -1, W).bfloat16() for t_ in (q, k))
+        v = rn(B, nkv, W).bfloat16()
+    for b in range(B):
+        x = score_range(q[b], k[b], heads, D, scale)
+        assert x < EXP2_DOMAIN, f"{dist}: |scale log2(e) q.k| reaches {x:.1f}, outside the domain of E_EXP"
+    return q, k, v
+
+
+def emulate_attn(q, k, v, scale, tile, fault=None):
+    """fp32 emulation of the wgmma flash kernels for one head (q [nq, D], k / v [nkv, D] bf16) over `tile`-key tiles (128 for
+    attention_d64_kernel, 64 for attention_kernel<D>), in the kernels' arrangement: a query row lives in the 4 lanes of a quad, lane j
+    holding keys and output columns with (index mod 8) // 2 == j; each lane keeps the running maximum m (exp2 units), its partial row
+    sum l from the fp32 P, and its O columns, which P rounded to bf16 times V accumulates into.  Per tile: m' = max(m, tile row max),
+    alpha = exp2(m - m'), P = exp2(s scale log2(e) - m'), l = alpha l + sum P, O = alpha O + P V.  The output is O / (sum of the 4 l).
+    The faults:
+      "padded"  every padded key of the last tile (zero-filled K and V: score 0) enters the softmax;
+      "mask"    the ragged mask is off by one and admits key nkv (zero-filled: score 0);
+      "l" / "o" a new running maximum does not rescale l / O;
+      "late"    the alpha of tile j + 1 is applied before P_j V_j is added, so P_j V_j escapes one rescale;
+      "quad"    the running maximum is taken per lane, without the reduction over the quad."""
+    nq, D = q.shape
+    nkv = k.shape[0]
+    nt = -(-nkv // tile)
+    kp = torch.zeros((nt * tile, D), dtype=torch.float32)
+    vp = torch.zeros_like(kp)
+    kp[:nkv], vp[:nkv] = k.float(), v.float()
+    valid = nt * tile if fault == "padded" else nkv + 1 if fault == "mask" else nkv
+    lane_k, lane_c = (torch.arange(tile) % 8) // 2, (torch.arange(D) % 8) // 2
+    c = float(torch.tensor(scale, dtype=torch.float32) * torch.tensor(L2E, dtype=torch.float32))  # scale_log2, rounded to fp32
+    m = torch.full((nq, 4), -float("inf"))
+    l = torch.zeros((nq, 4))
+    acc = torch.zeros((nq, D))
+    pend = torch.zeros((nq, D))
+    for t in range(nt):
+        s = q.float() @ kp[t * tile:(t + 1) * tile].t()
+        s[:, torch.arange(t * tile, (t + 1) * tile) >= valid] = -float("inf")
+        mx = torch.stack([s[:, lane_k == j].amax(1) for j in range(4)], 1) * c
+        if fault != "quad":
+            mx = mx.amax(1, keepdim=True).expand(-1, 4)
+        mn = torch.maximum(m, mx)
+        alpha = torch.exp2(m - mn)
+        p = torch.exp2(s * c - mn[:, lane_k])
+        psum = torch.stack([p[:, lane_k == j].sum(1) for j in range(4)], 1)
+        l = (l if fault == "l" else l * alpha) + psum
+        pv = p.bfloat16().float() @ vp[t * tile:(t + 1) * tile]
+        if fault == "o":
+            acc = acc + pv
+        elif fault == "late":
+            acc, pend = acc * alpha[:, lane_c] + pend, pv
+        else:
+            acc = acc * alpha[:, lane_c] + pv
+        m = mn
+    return ((acc + pend) / l.sum(1, keepdim=True)).bfloat16()
 
 
 def _lpd(v, cap):

@@ -289,16 +289,17 @@ def _attn_desc(**kw):
 
 
 ATTN_REJECT = {"out 2-byte aligned": ("out", "out"), "odd out_batch_stride": ("out_batch_stride", "out_batch_stride"),
-               "out_pitch below the head columns": ("out_pitch", "pitch")}
+               "out_pitch below the head columns": ("out_pitch", "pitch"), "q 8-byte aligned": ("q", "q 0x"),
+               "k_batch_stride not a multiple of 8": ("k_batch_stride", "k_batch_stride")}
 
 
-@pytest.mark.parametrize("entry", ["ladi_attention_bf16", "ladi_attention_d512_bf16"])
+@pytest.mark.parametrize("entry", ["ladi_attention_bf16", "ladi_attention_d512_bf16", "plan", "plan wide"])
 @pytest.mark.parametrize("name", list(ATTN_REJECT))
 def test_attention_placement_rejected(entry, name):
-    """Both entry points validate before they touch a device, so the rejection is visible here."""
+    """Both entry points and their plan query validate before they touch a device, so the rejection is visible here."""
     lib = ladi_lib().load()
     field, word = ATTN_REJECT[name]
-    if entry == "ladi_attention_d512_bf16":
+    if entry in ("ladi_attention_d512_bf16", "plan wide"):
         cols = 512
         d = _attn_desc(heads=1, head_dim=512, q_pitch=cols, k_pitch=cols, v_pitch=cols, out_pitch=cols, q_batch_stride=cols * 100,
                        k_batch_stride=cols * 77, v_batch_stride=cols * 77, out_batch_stride=cols * 100)
@@ -307,12 +308,19 @@ def test_attention_placement_rejected(entry, name):
         d = _attn_desc()
     if field == "out":
         d.out += 2
+    elif field == "q":
+        d.q += 8
     elif field == "out_batch_stride":
         d.out_batch_stride += 1
+    elif field == "k_batch_stride":
+        d.k_batch_stride += 4
     else:
         d.out_pitch = cols // 2
     before = lib.ladi_launch_count()
-    assert getattr(lib, entry)(C.byref(d), None) == 1
+    if entry.startswith("plan"):
+        assert lib.ladi_attention_plan(C.byref(d), int(entry == "plan wide"), 132, C.byref(ladi_lib().AttnPlan())) == 1
+    else:
+        assert getattr(lib, entry)(C.byref(d), None) == 1
     assert word in lib.ladi_last_error().decode()
     assert lib.ladi_launch_count() == before
 

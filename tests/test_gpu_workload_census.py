@@ -28,8 +28,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from kernel_check import (U_BF16, Replay, argworst, attn_expect, attn_ref, census, check_cls, conv_expect, determinism, flat_buf, layout,
-                          norm_expect, norm_input, pick, ptr, ratio, replay_conv, replay_ln, twice)
+from kernel_check import (U_BF16, Replay, argworst, attn_expect, attn_ref, census, check_cls, conv_expect, determinism, emulate_attn, flat_buf,
+                          layout, norm_expect, norm_input, pick, ptr, ratio, replay_conv, replay_ln, twice)
 
 # ================================================================================================================ the census (CPU)
 # per op: the fields the trace prints; the replay implements exactly these (an unknown op or field fails test_census_integrity)
@@ -282,54 +282,12 @@ def _attn_case(seed, nq, nkv, D=64):
     return q, k, v, o, sv
 
 
-def _emulate_attn(q, k, v, scale, padded_keys_count=False, tile=128, skip_rescale=None):
-    """Flash-style fp32 emulation over K/V tiles of 128: running max, exp2, P rounded to bf16 for P.V, l from the fp32 P.  The faults:
-    the padded keys of the last tile (zero-filled K and V) enter the softmax as keys of score 0; skip_rescale = "l" / "o": a new running
-    maximum does not rescale l / the O accumulator."""
-    nkv = k.shape[0]
-    nt = -(-nkv // tile)
-    kp = torch.zeros((nt * tile, k.shape[1]), dtype=torch.float32)
-    vp = torch.zeros_like(kp)
-    kp[:nkv], vp[:nkv] = k.float(), v.float()
-    mx = torch.full((q.shape[0], 1), -float("inf"))
-    l = torch.zeros((q.shape[0], 1))
-    acc = torch.zeros((q.shape[0], k.shape[1]))
-    l2e = 1.4426950408889634
-    for t in range(nt):
-        s = (q.float() @ kp[t * tile:(t + 1) * tile].t()) * (scale * l2e)
-        if not padded_keys_count:
-            valid = torch.arange(t * tile, (t + 1) * tile) < nkv
-            s[:, ~valid] = -float("inf")
-        mn = torch.maximum(mx, s.amax(1, keepdim=True))
-        p = torch.exp2(s - mn)
-        corr = torch.exp2(mx - mn)
-        l = (l if skip_rescale == "l" else l * corr) + p.sum(1, keepdim=True)
-        acc = (acc if skip_rescale == "o" else acc * corr) + p.bfloat16().float() @ vp[t * tile:(t + 1) * tile]
-        mx = mn
-    return (acc / l).bfloat16()
-
-
 @pytest.mark.parametrize("nkv", [77, 200])
 def test_bound_attention_teeth(nkv):
     q, k, v, o, sv = _attn_case(3, 96, nkv)
     bound = attn_expect(o, sv, nkv)
-    assert float(ratio(_emulate_attn(q, k, v, 0.125), o, bound).max()) <= 1.0  # honest: accepted
-    assert float(ratio(_emulate_attn(q, k, v, 0.125, padded_keys_count=True), o, bound).max()) > 1  # 5. padded keys counted: rejected
-
-
-@pytest.mark.parametrize("skip", ["l", "o"])
-def test_bound_attention_rescale_teeth(skip):
-    """Keys whose scores grow tile by tile (the maximum moves on every tile): skipping the rescale of l or of O is rejected."""
-    g = torch.Generator().manual_seed(4)
-    D, nq, nkv = 64, 96, 64 * 6
-    u = torch.sign(torch.randn(D, generator=g))
-    q = (torch.randn((nq, D), generator=g) * 0.5 + u).bfloat16()
-    k = (torch.randn((nkv, D), generator=g) * 0.5 + (2.0 * (torch.arange(nkv) // 64) / (0.125 * D))[:, None] * u).bfloat16()
-    v = torch.randn((nkv, D), generator=g).bfloat16()
-    o, sv = attn_ref(q.double(), k.double(), v.double(), 1, D, 0.125)
-    bound = attn_expect(o, sv, nkv)
-    assert float(ratio(_emulate_attn(q, k, v, 0.125, tile=64), o, bound).max()) <= 1.0
-    assert float(ratio(_emulate_attn(q, k, v, 0.125, tile=64, skip_rescale=skip), o, bound).max()) > 1
+    assert float(ratio(emulate_attn(q, k, v, 0.125, 128), o, bound).max()) <= 1.0  # honest: accepted
+    assert float(ratio(emulate_attn(q, k, v, 0.125, 128, "padded"), o, bound).max()) > 1  # 5. padded keys counted: rejected
 
 
 # ================================================================================================================ GPU: replay
